@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — CogView-base 4B hot path on B200 (BASELINE.json metric: tokens/sec, train + AR sample).
+"""bench.py — CogView-base 4B hot path on H100 (BASELINE.json metric: tokens/sec, train + AR sample).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload sample|train|both]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
@@ -9,8 +10,10 @@ Headline line (`value`, `e2e`): BASELINE.json configs[1] — 4B (48 L, d=2560, 4
 sequences, bf16, autoregressive sampling through the reference-facing API (generation.sampling.filling_sequence
 over GPT2Model): one step = prefill a 65-token context and generate 1024 image tokens for a batch of 4 beams
 (scripts/text2image.sh defaults).  The same JSON line carries a `train` object for configs[2] (one optimizer
-step on 4 x 1088 tokens per GPU: forward, vocab cross-entropy, backward, DP gradient all-reduce, fused AdamW).
-Synthetic tokens, random-init weights (no network for checkpoints).  `--impl reference` times the reference's
+step on 2 x 1088 tokens per GPU: forward, vocab cross-entropy, backward, DP gradient all-reduce, fused AdamW).
+Synthetic tokens, random-init weights (no network for checkpoints), all drawn from fixed seeds: the same arguments
+give the same inputs on every run, and --dump-outputs DIR writes what the last timed step of each workload computed
+(DIR/<workload>_<name>.npy, float32 / float64) so that two builds can be compared output for output.  `--impl reference` times the reference's
 own modules (oracle/_ref, placed by oracle/build_ref.py; hidden-state `mems` semantics) on the host cores — or the
 oracle port when oracle/_ref is absent.  The driver's record keeps only the contract keys of the JSON line, so the
 training / VQ-VAE results are also summarised inside `config` (`config.train`, `config.vqvae`).
@@ -42,7 +45,10 @@ def parse():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default="all", choices=["sample", "train", "vqvae", "both", "all"])
     ap.add_argument("--vq-batch", type=int, default=256)
-    ap.add_argument("--batch", type=int, default=4, help="beams per GPU (sampling) / sequences per GPU (training)")
+    ap.add_argument("--batch", type=int, default=4, help="beams per GPU (sampling)")
+    # 80 GB per GPU: the 4B model's bf16 weights and gradients, fp32 master weights and AdamW moments take ~62 GB, which
+    # leaves room for the activations of 2 x 1088 tokens (no activation recompute), not of 4
+    ap.add_argument("--train-batch", type=int, default=2, help="sequences per GPU (training)")
     ap.add_argument("--gen-tokens", type=int, default=1024)
     ap.add_argument("--model", default="4b", choices=["4b", "tiny"])
     ap.add_argument("--train-steps", type=int, default=None)
@@ -50,17 +56,9 @@ def parse():
                     help="development only: leave out the host-core baseline leg (the default run includes it)")
     ap.add_argument("--dropout", type=float, default=0.1,
                     help="embedding/attention/hidden dropout of the training workload (reference scripts: 0.1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step of each workload to DIR/<name>.npy")
     return ap.parse_args()
-
-
-def measured_traffic(kernel):
-    """DRAM bytes per launch from the committed ncu captures (profiles/r02_traffic.json, r01_traffic.json), or None."""
-    for name in ("r02_traffic.json", "r01_traffic.json"):
-        try:
-            return json.load(open(os.path.join(ROOT, "profiles", name)))[kernel]["traffic_bytes_per_launch"]
-        except Exception:
-            continue
-    return None
 
 
 def peaks():
@@ -69,7 +67,8 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sust=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     src="measured (MEASURED_PEAKS.json)")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sust=1400.0, src="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 — a ceiling, not a reached rate
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sust=989.0, src="H100 SXM data sheet")
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -232,6 +231,7 @@ def run_sample(args, cfg, world, rank, dev_index):
                e2e=dict(value=tokens_per_step * args.steps / (ms_e2e / 1e3), unit="tokens/s",
                         h2d_bytes_per_step=int(tmpl_host.numel() * 8), d2h_bytes_per_step=int(out_host.numel() * 8)),
                gpu_launches=int(n_launch / max(1, (args.steps + args.warmup))) * args.steps)
+    res["outputs"] = dict(tokens=holder["out"])
     res["roofline"] = sample_roofline(model, nb, res["ms_per_step"], args.gen_tokens)
     res["params"] = param_count(model)
     del model
@@ -243,7 +243,7 @@ def sample_roofline(model, nb, ms_per_step, gen_tokens, ctx_len=65):
     """Dominant decode kernel = decode_step_kernel (one launch per token: all layers + logits, weight streaming).
     Algorithmic bytes per launch (SURVEY §8(d)): every bf16 weight once (7.858 GB) + the K|V rows of the cached
     tokens (491,520 B x t per sequence).  Timed live with CUDA events over launches of the kernel alone at the mean
-    memory length of the generation (each launch streams 7.9 GB >> the 126 MB L2, so nothing is served from cache)."""
+    memory length of the generation (each launch streams 7.9 GB >> the 50 MB L2, so nothing is served from cache)."""
     from cogview_b200 import ops
     from cogview_b200.mpu import kv_cache
     from cogview_b200.mpu.decode import DecodeRunner
@@ -288,7 +288,7 @@ def sample_roofline(model, nb, ms_per_step, gen_tokens, ctx_len=65):
         achieved = wbytes / (ms / 1e3) / 1e9
         del r, c
         return dict(kernel="linear_small_m_kernel", bound="hbm", achieved=achieved, peak=pk["hbm"], unit="GB/s",
-                    frac=achieved / pk["hbm"], traffic=measured_traffic("linear_small_m_kernel"), peak_source=pk["src"],
+                    frac=achieved / pk["hbm"], peak_source=pk["src"],
                     launches_per_step=n_l * gen_tokens, bytes_per_launch=wbytes / n_l, avg_launch_us=ms * 1e3 / n_l,
                     share_of_step=ms * gen_tokens / ms_per_step,
                     note="algorithmic bytes = the weight matrix of each launch (mean %.1f MB; all %d launches of a token "
@@ -315,7 +315,7 @@ def sample_roofline(model, nb, ms_per_step, gen_tokens, ctx_len=65):
     achieved = nbytes / (ms / 1e3) / 1e9
     del r, c
     return dict(kernel="decode_step_kernel", bound="hbm", achieved=achieved, peak=pk["hbm"], unit="GB/s",
-                frac=achieved / pk["hbm"], traffic=measured_traffic("decode_step_kernel"), peak_source=pk["src"],
+                frac=achieved / pk["hbm"], peak_source=pk["src"],
                 launches_per_step=gen_tokens, bytes_per_launch=nbytes, avg_launch_us=ms * 1e3,
                 share_of_step=ms * gen_tokens / ms_per_step,
                 note="bytes = all weights + K|V of t=%d cached tokens x %d seqs; share_of_step = kernel x tokens / step" % (
@@ -338,16 +338,14 @@ def run_train(args, cfg, world, rank, dev_index, steps, warmup):
     reserved = 0
     if world > 1:
         # the gradient all-reduce (pretrain_gpt2.py:99-105) runs as NCCL kernels NEXT TO the backward GEMMs: keep a few
-        # SMs out of the persistent GEMM grid for them (a grid sized to all 148 SMs would find some taken and run a
-        # second, nearly empty wave), and cap NCCL's CTAs to what was reserved (main() sets NCCL_MAX_CTAS).  Measured at
-        # N = 2 (4 x 1088 tokens per GPU): 182.4 ms with nothing reserved (NCCL up to 32 CTAs), 183.0 ms with 16, 180.1 ms
-        # with 8 (N = 1: 166.9 ms) — profiles/r02_train_2gpu_reserved_sms.txt
+        # SMs out of the persistent GEMM grid for them (a grid sized to all SMs would find some taken and run a
+        # second, nearly empty wave), and cap NCCL's CTAs to what was reserved (main() sets NCCL_MAX_CTAS)
         from cogview_b200 import _lib
         reserved = int(os.environ.get("COGVIEW_B200_RESERVE_SMS", "8"))
         _lib.lib().cv_set_reserved_sms(reserved)
         net = PyTorchDistributedDataParallel(model, device_ids=[torch.cuda.current_device()],
                                              gradient_as_bucket_view=True, bucket_cap_mb=200)
-    b, s = args.batch, cfg["max_sequence_length"] - 1
+    b, s = args.train_batch, cfg["max_sequence_length"] - 1
     g = torch.Generator().manual_seed(100 + rank)
     host_tokens = torch.cat((torch.randint(8192, 58192, (b, 64), generator=g),
                              torch.randint(0, 8192, (b, s + 1 - 64), generator=g)), dim=1).pin_memory()
@@ -399,8 +397,9 @@ def run_train(args, cfg, world, rank, dev_index, steps, warmup):
                step_flops_per_gpu=flops_per_token * tokens_per_step / world,
                roofline_step=dict(bound="tensor", achieved=achieved, peak=pk["tf_sust"], unit="TFLOP/s",
                                   frac=achieved / pk["tf_sust"], peak_source=pk["src"],
-                                  note="whole step (all kernels) vs sustained cuBLAS bf16 peak"))
+                                  note="whole step (all kernels) vs the data-sheet dense bf16 peak"))
     res["config"]["reserved_sms_for_nccl"] = reserved
+    res["outputs"] = dict(loss=last["loss"].detach())
     if world > 1:
         from cogview_b200 import _lib
         _lib.lib().cv_set_reserved_sms(0)
@@ -411,7 +410,7 @@ def run_train(args, cfg, world, rank, dev_index, steps, warmup):
 
 
 def gemm_roofline(cfg, M):
-    """Dominant training kernel = gemm_kernel (tcgen05).  FLOPs per launch = 2*M*N*K; timed live with CUDA events
+    """Dominant training kernel = gemm_kernel (wgmma).  FLOPs per launch = 2*M*N*K; timed live with CUDA events
     over the four forward GEMM shapes of a layer, rotating through 6 weight sets (> L2)."""
     from cogview_b200 import ops
     pk = peaks()
@@ -440,9 +439,7 @@ def gemm_roofline(cfg, M):
         del ws, x
     achieved = tot_f / tot_ms / 1e9
     return dict(kernel="gemm_kernel", bound="tensor", achieved=achieved, peak=pk["tf_burst"], unit="TFLOP/s",
-                frac=achieved / pk["tf_burst"], traffic=measured_traffic("gemm_kernel"),
-                traffic_note="ncu capture of the qkv shape (profiles/r01_traffic.json): operands read once",
-                peak_source=pk["src"], shapes=out,
+                frac=achieved / pk["tf_burst"], peak_source=pk["src"], shapes=out,
                 flops_per_launch=tot_f / n, avg_launch_us=tot_ms * 1e3 / n)
 
 
@@ -493,10 +490,37 @@ def run_vqvae(args, world, rank, dev_index, steps, warmup):
                            parallelism="dp%d (independent images per rank, no collective)" % world),
                roofline_step=dict(bound="tensor", achieved=achieved, peak=pk["tf_sust"], unit="TFLOP/s",
                                   frac=achieved / pk["tf_sust"], peak_source=pk["src"],
-                                  note="whole round trip (224.6 GFLOP/image algorithmic) vs sustained cuBLAS bf16 peak"))
+                                  note="whole round trip (224.6 GFLOP/image algorithmic) vs the data-sheet dense bf16 peak"))
+    res["outputs"] = dict(codes=keep["codes"], recon=keep["rec"])
     del model
     torch.cuda.empty_cache()
     return res
+
+
+DUMP_LIMIT = 64 << 20     # bytes written by --dump-outputs in all
+SAMPLE_ELEMS = 1 << 20    # larger outputs are dumped as a fixed, seeded sample of this many elements
+
+
+def dump_outputs(dirname, outputs):
+    """outputs: {name: tensor}.  Integer outputs are written as float64 (exact), floating ones as float32; an output
+    with more than SAMPLE_ELEMS elements is written as the elements at seeded random flat indices (the indices go to
+    <name>_index.npy), so the files stay well inside DUMP_LIMIT."""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    total = 0
+    for name, t in sorted(outputs.items()):
+        t = t.detach().reshape(-1)
+        if t.numel() > SAMPLE_ELEMS:
+            g = torch.Generator().manual_seed(0)
+            idx = torch.randperm(t.numel(), generator=g)[:SAMPLE_ELEMS].sort().values
+            np.save(os.path.join(dirname, name + "_index.npy"), idx.numpy().astype(np.float64))
+            total += idx.numel() * 8
+            t = t[idx.to(t.device)]
+        arr = t.cpu().numpy().astype(np.float32 if t.is_floating_point() else np.float64)
+        total += arr.nbytes
+        if total > DUMP_LIMIT:
+            raise SystemExit("--dump-outputs: outputs exceed %d bytes" % DUMP_LIMIT)
+        np.save(os.path.join(dirname, name + ".npy"), arr)
 
 
 def usable_cores():
@@ -782,7 +806,7 @@ def main():
                      "kernel, one CUDA-graph replay per token" % (args.gen_tokens, args.batch))
     # BASELINE.json's metric; `value` is the AR-sampling tokens/s (configs[1]), the training step (configs[2]) and the
     # VQ-VAE round trip (configs[3]) are summarised in config.train / config.vqvae and in full in `train` / `vqvae`
-    base = dict(metric="tokens/sec (train + AR sample) CogView-4B seq1089 @1/2/4/8 B200; %roofline", unit="tokens/s",
+    base = dict(metric="tokens/sec (train + AR sample) CogView-4B seq1089 @1/2/4/8 H100; %roofline", unit="tokens/s",
                 n_gpus=world, steps=args.steps, warmup=args.warmup, higher_is_better=True, scaling="weak",
                 vs_baseline=None, dtype="bf16", data="synthetic tokens, random-init weights")
 
@@ -825,15 +849,19 @@ def main():
         mpu.initialize_model_parallel(1)
 
     line = dict(base)
+    outputs = {}
     if args.workload in ("sample", "both", "all"):
+        torch.manual_seed(1000 + rank)      # weights and the sampling draws
         r = run_sample(args, cfg, world, rank, local_rank)
+        outputs.update(("sample_" + k, x) for k, x in r.pop("outputs").items())
         line.update(value=r["value"], ms_per_step=r["ms_per_step"], e2e=r["e2e"], clocks=r["clocks"],
                     gpu_launches=r["gpu_launches"], roofline=r["roofline"],
                     config=dict(workload=workload_name, global_batch=args.batch * world, seq_len=1089,
                                 parallelism="dp%d (independent sequences per rank, no collective)" % world,
-                                l2="each decode step streams 7.9 GB of weights (>> 126 MB L2)", params=r["params"]))
+                                l2="each decode step streams 7.9 GB of weights (>> 50 MB L2)", params=r["params"]))
     if args.workload in ("vqvae", "all"):
-        v = run_vqvae(args, world, rank, local_rank, max(3, args.steps), max(3, args.warmup))
+        torch.manual_seed(2000 + rank)
+        v = run_vqvae(args, world, rank, local_rank, args.steps, args.warmup)
         if args.workload == "vqvae":
             line.update(metric="images/sec (VQ-VAE encode+quantise+decode, 256x256)", unit="images/s", value=v["value"],
                         ms_per_step=v["ms_per_step"], e2e=v["e2e"], clocks=v["clocks"], gpu_launches=v["gpu_launches"],
@@ -841,10 +869,12 @@ def main():
         else:
             line["config"]["vqvae"] = dict(value=v["value"], unit="images/s", ms_per_step=v["ms_per_step"],
                                            frac_of_sustained_tensor_peak=v["roofline_step"]["frac"])
+        outputs.update(("vqvae_" + k, x) for k, x in v.pop("outputs").items())
         line["vqvae"] = v
     if args.workload in ("train", "both", "all"):
-        tsteps = args.train_steps or max(3, args.steps)
-        t = run_train(args, cfg, world, rank, local_rank, tsteps, max(3, args.warmup))
+        tsteps = args.train_steps or args.steps
+        torch.manual_seed(3000 + rank)
+        t = run_train(args, cfg, world, rank, local_rank, tsteps, args.warmup)
         if args.workload == "train":
             line.update(metric="tokens/sec (train) CogView-4B seq1089", value=t["value"], ms_per_step=t["ms_per_step"],
                         e2e=t["e2e"], clocks=t["clocks"], gpu_launches=t["gpu_launches"], roofline=t["roofline"],
@@ -857,7 +887,10 @@ def main():
                                            step_frac_of_sustained_tensor_peak=t["roofline_step"]["frac"],
                                            gemm_frac_of_burst_peak=t["roofline"]["frac"], loss=t["loss"],
                                            exposed_comm_ms=t.get("exposed_comm_ms"))
+        outputs.update(("train_" + k, x) for k, x in t.pop("outputs").items())
         line["train"] = t
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, outputs)
     if rank == 0 and (args.skip_cpu_baseline or world > 1):
         # the CPU baseline is reported at N = 1 only (--skip-cpu-baseline: development runs)
         line["cpu_baseline"] = None

@@ -7,15 +7,16 @@
 //   dV = P^T dO        dP = dO V^T        dS = P o (dP - D),  D = rowsum(dO o O)
 //   dQ = scale * dS K  dK = scale * dS^T Q
 //
-// One CTA per (128-key block, head, batch) loops over the query blocks that can see it.  All five products
-// run on tcgen05 with TMEM accumulators; every operand is used in place from 128B-swizzled TMA tiles, in
-// K-major or MN-major form as the product needs (the same Q / dO / K tiles serve both):
+// One CTA per (128-key block, head, batch) loops over the query blocks that can see it: a TMA producer warpgroup
+// and two wgmma warpgroups that own 64 key rows each.  All five products run on wgmma with fp32 accumulators in
+// registers; the shared-memory operands are used in place from 128B-swizzled TMA tiles, in K-major or MN-major
+// form as the product needs (the same Q / dO / K tiles serve both):
 //   S^T  = K Q^T      (A = K   K-major, B = Q  K-major)   [keys x queries]
 //   dP^T = V dO^T     (A = V   K-major, B = dO K-major)
-//   dV  += P^T dO     (A = P^T K-major (smem, written by the softmax warps), B = dO MN-major)
-//   dK  += dS^T Q     (A = dS^T K-major (smem),                               B = Q  MN-major)
-//   dQ_i = dS K       (A = dS^T read MN-major,                                B = K  MN-major)
-// dV / dK stay in TMEM for the whole loop; dQ tiles are reduced into an fp32 buffer with vector red.add.
+//   dV  += P^T dO     (A = P^T from registers,  B = dO MN-major)
+//   dK  += dS^T Q     (A = dS^T from registers, B = Q  MN-major)
+//   dQ_i = dS K       (A = dS^T of both warpgroups, written to smem and read MN-major, B = K MN-major)
+// dV / dK stay in registers for the whole loop; dQ tiles are reduced into an fp32 buffer with vector red.add.
 #include "common.cuh"
 #include "host.h"
 #include "../../include/cogview_b200.h"
@@ -28,10 +29,10 @@ constexpr int HD = 64;
 constexpr int TILE_BYTES = BLK * HD * 2;      // 16 KB: one [128 x 64] bf16 tile
 constexpr int PT_BYTES = BLK * BLK * 2;       // 32 KB: [128 keys x 128 queries] bf16
 constexpr int QDO_STAGES = 2;
-constexpr int SMEM_BYTES = 2 * TILE_BYTES /*K,V*/ + QDO_STAGES * 2 * TILE_BYTES /*Q,dO*/ + 2 * PT_BYTES /*P^T,dS^T*/ +
-                           QDO_STAGES * 3 * BLK * 4 /*lse2, D, band start*/ + 1024 + 256;
+constexpr int SMEM_BYTES = 2 * TILE_BYTES /*K,V*/ + QDO_STAGES * 2 * TILE_BYTES /*Q,dO*/ + 2 * PT_BYTES /*dS^T x 2*/ +
+                           2 * 2 * 3 * BLK * 4 /*per warpgroup, 2 buffers: lse2, D, band start*/ + 1024 + 256;
 enum { MODE_DENSE = 0, MODE_BAND = 1, MODE_PIVOT = 2 };
-constexpr int NUM_THREADS = 320;     // TMA warp, MMA warp, 8 compute warps (two threads per key row)
+constexpr int NUM_THREADS = 384;     // TMA warpgroup, two wgmma warpgroups (64 key rows each)
 constexpr float LOG2E = 1.4426950408889634f;
 
 struct BwdParams {
@@ -59,9 +60,8 @@ __device__ __forceinline__ int band_start(int i, int w, int times) {
     return g > 0 ? g * w : 0;
 }
 
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
-    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d)
-                 : "memory");
+__device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
+    asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
 }
 
 template <int MODE>
@@ -73,23 +73,14 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     uint8_t* sK = smem;
     uint8_t* sV = sK + TILE_BYTES;
     uint8_t* sQDO = sV + TILE_BYTES;                               // stage s: Q then dO
-    uint8_t* sPT = sQDO + QDO_STAGES * 2 * TILE_BYTES;
-    uint8_t* sDST = sPT + PT_BYTES;
-    float* sLse = reinterpret_cast<float*>(sDST + PT_BYTES);       // [stages][128]
-    float* sDelta = sLse + QDO_STAGES * BLK;
-    int* sBand = reinterpret_cast<int*>(sDelta + QDO_STAGES * BLK);   // [stages][128] band_start of the tile's queries
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sBand + QDO_STAGES * BLK);
+    uint8_t* sDST = sQDO + QDO_STAGES * 2 * TILE_BYTES;            // [2 buffers] dS^T [128 keys x 128 queries]
+    float* sStat = reinterpret_cast<float*>(sDST + 2 * PT_BYTES);  // [warpgroup][buffer][lse2 | D | band] x 128
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sStat + 2 * 2 * 3 * BLK);
     uint64_t* kv_full = bars;                  // 1
     uint64_t* qdo_full = bars + 1;             // [2]
-    uint64_t* qdo_empty = qdo_full + QDO_STAGES;
-    uint64_t* sdp_full = qdo_empty + QDO_STAGES;   // 1: S^T and dP^T ready in TMEM
-    uint64_t* pds_full = sdp_full + 1;             // 1: P^T / dS^T written to smem (and S^T/dP^T TMEM consumed)
-    uint64_t* pds_free = pds_full + 1;             // 1: MMAs reading P^T / dS^T smem retired
-    uint64_t* dq_full = pds_free + 1;              // 1
-    uint64_t* dq_free = dq_full + 1;               // 1
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(dq_free + 1);
+    uint64_t* qdo_empty = qdo_full + QDO_STAGES;   // [2]: one arrive per consumer warp
 
-    const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
     const int kb = blockIdx.x, head = blockIdx.y, batch = blockIdx.z;
     const int k0 = kb * BLK;
     const int nqb = (p.s + BLK - 1) / BLK;
@@ -103,33 +94,24 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     }
     const int ntiles = i_end - i_start + 1;
 
-    if (warp_idx == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV); tma_prefetch_desc(&tmDO);
         mbar_init(kv_full, 1);
-        for (int i = 0; i < QDO_STAGES; ++i) { mbar_init(&qdo_full[i], 1); mbar_init(&qdo_empty[i], 1); }
-        mbar_init(sdp_full, 1);
-        mbar_init(pds_full, 256);
-        mbar_init(pds_free, 1);
-        mbar_init(dq_full, 1);
-        mbar_init(dq_free, 256);
+        for (int i = 0; i < QDO_STAGES; ++i) { mbar_init(&qdo_full[i], 1); mbar_init(&qdo_empty[i], 8); }
         fence_barrier_init();
     }
-    if (warp_idx == 1) tmem_alloc<512>(tmem_ptr);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
-    constexpr uint32_t TM_ST = 0, TM_DPT = 128, TM_DV = 256, TM_DK = 320, TM_DQ = 384;
 
-    if (warp_idx == 0) {
-        if (lane == 0) {
+    if (wg == 0) {
+        setmaxnreg_dec<40>();
+        if (tid == 0) {
             mbar_expect_tx(kv_full, 2 * TILE_BYTES);
             tma_load_3d(sK, &tmK, kv_full, head * HD, k0, batch);
             tma_load_3d(sV, &tmV, kv_full, head * HD, k0, batch);
             int stage = 0; uint32_t phase = 0;
             for (int t = 0; t < ntiles; ++t) {
                 const int q0 = (i_start + t) * BLK;
-                mbar_wait(&qdo_empty[stage], phase ^ 1);
+                mbar_wait<false>(&qdo_empty[stage], phase ^ 1);
                 uint8_t* sQ = sQDO + stage * 2 * TILE_BYTES;
                 mbar_expect_tx(&qdo_full[stage], 2 * TILE_BYTES);
                 tma_load_3d(sQ, &tmQ, &qdo_full[stage], head * HD, q0, batch);
@@ -137,253 +119,178 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
                 if (++stage == QDO_STAGES) { stage = 0; phase ^= 1; }
             }
         }
-    } else if (warp_idx == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc_s = make_idesc_bf16(BLK, BLK, 0, 0);
-            constexpr uint32_t idesc_acc = make_idesc_bf16(BLK, HD, 0, 1);   // A K-major (smem P^T/dS^T), B MN-major
-            constexpr uint32_t idesc_dq = make_idesc_bf16(BLK, HD, 1, 1);    // A MN-major (dS^T read as dS), B MN-major
-            const uint32_t k_addr = smem_u32(sK), v_addr = smem_u32(sV);
-            const uint32_t pt_addr = smem_u32(sPT), dst_addr = smem_u32(sDST);
-            auto issue_sdp = [&](int stage) {
-                const uint32_t q_addr = smem_u32(sQDO + stage * 2 * TILE_BYTES);
-                const uint32_t do_addr = q_addr + TILE_BYTES;
-#pragma unroll
-                for (int k = 0; k < HD / 16; ++k)
-                    umma_f16(tmem_base + TM_ST, make_smem_desc_sw128(k_addr + k * 32, 0, 1024),
-                             make_smem_desc_sw128(q_addr + k * 32, 0, 1024), idesc_s, k != 0);
-#pragma unroll
-                for (int k = 0; k < HD / 16; ++k)
-                    umma_f16(tmem_base + TM_DPT, make_smem_desc_sw128(v_addr + k * 32, 0, 1024),
-                             make_smem_desc_sw128(do_addr + k * 32, 0, 1024), idesc_s, k != 0);
-                umma_commit(sdp_full);
-            };
-            mbar_wait(kv_full, 0);
-            int stage = 0; uint32_t phase = 0;
-            mbar_wait(&qdo_full[0], 0);
-            tc_fence_after();
-            issue_sdp(0);
-            for (int t = 0; t < ntiles; ++t) {
-                mbar_wait(pds_full, t & 1);           // P^T / dS^T in smem; S^T / dP^T TMEM consumed
-                if (t > 0) mbar_wait(dq_free, (t - 1) & 1);   // previous dQ tile drained from TMEM
-                tc_fence_after();
-                const uint32_t q_addr = smem_u32(sQDO + stage * 2 * TILE_BYTES);
-                const uint32_t do_addr = q_addr + TILE_BYTES;
-                // dQ first: the softmax warps are waiting for it, and its read-out (TMEM -> red.add) then overlaps dV / dK
-#pragma unroll
-                for (int k = 0; k < BLK / 16; ++k)     // reduction over the 128 keys of this block
-                    umma_f16(tmem_base + TM_DQ, make_smem_desc_sw128(dst_addr + k * 2048, BLK * 128, 1024),
-                             make_smem_desc_sw128(k_addr + k * 2048, BLK * 128, 1024), idesc_dq, k != 0);
-                umma_commit(dq_full);
-#pragma unroll
-                for (int k = 0; k < BLK / 16; ++k) {   // reduction over the 128 queries of this tile
-                    const uint32_t a_off = (k >> 2) * (BLK * 128) + (k & 3) * 32;
-                    umma_f16(tmem_base + TM_DV, make_smem_desc_sw128(pt_addr + a_off, 0, 1024),
-                             make_smem_desc_sw128(do_addr + k * 2048, BLK * 128, 1024), idesc_acc, (t | k) != 0);
-                    umma_f16(tmem_base + TM_DK, make_smem_desc_sw128(dst_addr + a_off, 0, 1024),
-                             make_smem_desc_sw128(q_addr + k * 2048, BLK * 128, 1024), idesc_acc, (t | k) != 0);
-                }
-                umma_commit(&qdo_empty[stage]);
-                umma_commit(pds_free);
-                if (++stage == QDO_STAGES) { stage = 0; phase ^= 1; }
-                if (t + 1 < ntiles) {
-                    mbar_wait(&qdo_full[stage], phase);
-                    tc_fence_after();
-                    issue_sdp(stage);
-                }
-            }
-        }
     } else {
-        // 8 warps: warp w works on TMEM lane quadrant w % 4 (key rows 32 (w % 4) .. +31, one per lane); warps 2-5 take
-        // query columns 0-63 of every tile (and dQ / dK), warps 6-9 columns 64-127 (and dV): the per-tile chain of a
-        // thread is halved and every scheduler has two of these warps to overlap.  No exchange is needed between the two
-        // threads of a row — lse, delta and the band starts come from shared memory.
-        const int q = warp_idx & 3;
-        const int hf = (warp_idx - 2) >> 2;
-        const int row = q * 32 + lane;             // key row within the block
-        const int kj = k0 + row;
-        const int epi_tid = threadIdx.x - 64;      // 0..255; the first 128 stage the per-query statistics
-        const uint32_t lane_addr = tmem_base + (uint32_t(q * 32) << 16);
+        // Fragment layout (common.cuh): this thread holds key rows r_loc, r_loc + 8 of the block and, of every
+        // 8-query group of a tile, the two queries c_in, c_in + 1.  For dQ (rows = queries) the same positions index
+        // queries 64 half + ... and head dims.
+        setmaxnreg_inc<232>();
+        const int half = wg - 1, warp = tid >> 5, lane = tid & 31;
+        const int r_loc = 64 * half + 16 * warp + (lane >> 2);
+        const int c_in = 2 * (lane & 3);
         const float masked_val = -10000.0f * LOG2E;
-        const int my_pos = (MODE == MODE_PIVOT) ? (kj < p.sk ? p.piv_pos[(size_t)batch * p.sk + kj] : 0x7fffffff) : 0;
+        int kj[2], my_pos[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            kj[h] = k0 + r_loc + 8 * h;
+            my_pos[h] = (MODE == MODE_PIVOT) ? (kj[h] < p.sk ? p.piv_pos[(size_t)batch * p.sk + kj[h]] : 0x7fffffff) : 0;
+        }
         const size_t stat_base = ((size_t)batch * p.heads + head) * p.s;
         const size_t keep_base = ((size_t)batch * p.heads + head) * (size_t)nqb * BLK;   // key rows are padded to blocks
-        int stage = 0;
-        float pre_lse, pre_delta;
-        uint4 pre_keep = make_uint4(0, 0, 0, 0);
-        {
-            const int qn = i_start * BLK + (epi_tid & (BLK - 1));
-            pre_lse = (qn < p.s) ? p.lse[stat_base + qn] * LOG2E : 0.f;
-            pre_delta = (qn < p.s) ? p.delta[stat_base + qn] : 0.f;
-            if (p.drop_mask != nullptr)
-                pre_keep = *reinterpret_cast<const uint4*>(p.drop_mask + ((keep_base + kj) * (size_t)nqb + i_start) * 4);
-        }
+        const uint32_t k_addr = smem_u32(sK), v_addr = smem_u32(sV);
+        const uint32_t kh_addr = k_addr + half * (64 * 128), vh_addr = v_addr + half * (64 * 128);
+        float dv[HD / 2], dk[HD / 2];
+#pragma unroll
+        for (int i = 0; i < HD / 2; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
+        mbar_wait<false>(kv_full, 0);
+        int stage = 0; uint32_t phase = 0;
         for (int t = 0; t < ntiles; ++t) {
             const int q0 = (i_start + t) * BLK;
-            // lse (log2 domain), delta and keep bits of this query block were fetched one tile ahead (registers):
-            // publish them, then start the fetch for the next tile so its global-load latency is off the critical path
-            if (hf == 0) {
-                sLse[stage * BLK + epi_tid] = pre_lse;
-                sDelta[stage * BLK + epi_tid] = pre_delta;
-                if (MODE != MODE_DENSE) sBand[stage * BLK + epi_tid] = band_start(q0 + epi_tid, p.sp_w, p.sp_times);
+            const int buf = t & 1;
+            // per-query statistics of this tile (lse in the log2 domain, delta, band start) -> this warpgroup's buffer
+            float* st = sStat + (half * 2 + buf) * 3 * BLK;
+            {
+                const int qn = q0 + tid;
+                st[tid] = (qn < p.s) ? p.lse[stat_base + qn] * LOG2E : 0.f;
+                st[BLK + tid] = (qn < p.s) ? p.delta[stat_base + qn] : 0.f;
+                if (MODE != MODE_DENSE) reinterpret_cast<int*>(st)[2 * BLK + tid] = band_start(qn, p.sp_w, p.sp_times);
             }
-            const uint4 kw = pre_keep;                  // this key's keep bits over the 128 queries of the tile
-            if (t + 1 < ntiles) {
-                const int qn = q0 + BLK + (epi_tid & (BLK - 1));
-                pre_lse = (qn < p.s) ? p.lse[stat_base + qn] * LOG2E : 0.f;
-                pre_delta = (qn < p.s) ? p.delta[stat_base + qn] : 0.f;
-                if (p.drop_mask != nullptr)
-                    pre_keep = *reinterpret_cast<const uint4*>(p.drop_mask +
-                                                               ((keep_base + kj) * (size_t)nqb + i_start + t + 1) * 4);
+            uint4 kw[2] = {make_uint4(0u, 0u, 0u, 0u), make_uint4(0u, 0u, 0u, 0u)};
+            const bool use_drop = p.drop_mask != nullptr;
+            if (use_drop) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+                    kw[h] = *reinterpret_cast<const uint4*>(p.drop_mask + ((keep_base + kj[h]) * (size_t)nqb + i_start + t) * 4);
             }
-            named_bar_sync(1, 256);
-            mbar_wait(sdp_full, t & 1);
-            tc_fence_after();
-            if (t > 0) mbar_wait(pds_free, (t - 1) & 1);   // MMAs of the previous tile no longer read P^T / dS^T
+            named_bar_sync(1 + half, 128);
+            mbar_wait<false>(&qdo_full[stage], phase);
+            const uint32_t q_addr = smem_u32(sQDO + stage * 2 * TILE_BYTES);
+            const uint32_t do_addr = q_addr + TILE_BYTES;
+            float sacc[BLK / 2], dpacc[BLK / 2];
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < HD / 16; ++k)
+                wgmma_ss_n128<0, 0>(sacc, make_smem_desc_sw128(kh_addr + k * 32, 0, 1024),
+                                    make_smem_desc_sw128(q_addr + k * 32, 0, 1024), k != 0 ? 1u : 0u);
+            wgmma_commit();
+#pragma unroll
+            for (int k = 0; k < HD / 16; ++k)
+                wgmma_ss_n128<0, 0>(dpacc, make_smem_desc_sw128(vh_addr + k * 32, 0, 1024),
+                                    make_smem_desc_sw128(do_addr + k * 32, 0, 1024), k != 0 ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(sacc);
+            fence_regs(dpacc);
             bool full_vis = (q0 + BLK <= p.s) && (k0 + BLK <= p.s) &&
                             ((k0 + BLK <= p.sep_eff) || (k0 + BLK - 1 <= q0));
             if (MODE == MODE_BAND)      // every key of the block inside the band of every query of the tile
                 full_vis = (q0 + BLK <= p.s) && (k0 + BLK - 1 <= q0) &&
                            (k0 >= band_start(q0 + BLK - 1, p.sp_w, p.sp_times));
             if (MODE == MODE_PIVOT) full_vis = false;
-            const int* bnd = sBand + stage * BLK;
-            const float* lse2 = sLse + stage * BLK;
-            const float* dlt = sDelta + stage * BLK;
-            const bool use_drop = p.drop_mask != nullptr;
-            uint8_t* prow = sPT + row * 128;
-            uint8_t* drow = sDST + row * 128;
-#pragma unroll 2
-            for (int c = hf * 2; c < hf * 2 + 2; ++c) {      // this thread's 64 query columns
-                uint32_t sr[32], dr[32];
-                tmem_ld_x32(lane_addr + TM_ST + c * 32, sr);
-                tmem_ld_x32(lane_addr + TM_DPT + c * 32, dr);
-                tmem_ld_wait();
-                float pv[32], dv[32];
-                const uint32_t kwc = c == 0 ? kw.x : (c == 1 ? kw.y : (c == 2 ? kw.z : kw.w));
-                if (full_vis && use_drop) {            // interior tile with dropout: branch-free, bit i of kwc = query col
-                    const float ds = p.drop_scale;
+            const float* lse2 = st;
+            const float* dlt = st + BLK;
+            const int* bnd = reinterpret_cast<const int*>(st) + 2 * BLK;
+            uint32_t ppk[BLK / 4], dspk[BLK / 4];      // bf16 pairs of P^T (dropped) and dS^T, A-fragment order
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) {
-                        const int col = c * 32 + i;
-                        const bool keep = (kwc >> i) & 1u;
-                        const float pr = exp2f(__uint_as_float(sr[i]) * p.scale_log2 - lse2[col]);
-                        // dP flows back through the keep mask; dV sees the dropped probabilities
-                        const float dp = keep ? __uint_as_float(dr[i]) * ds : 0.f;
-                        pv[i] = keep ? pr * ds : 0.f;
-                        dv[i] = pr * (dp - dlt[col]) * p.scale;
-                    }
-                } else if (full_vis) {                 // interior tile, no dropout: branch-free inner loop
+            for (int i = 0; i < BLK / 8; ++i)
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) {
-                        const int col = c * 32 + i;
-                        const float pr = exp2f(__uint_as_float(sr[i]) * p.scale_log2 - lse2[col]);
-                        pv[i] = pr;
-                        dv[i] = pr * (__uint_as_float(dr[i]) - dlt[col]) * p.scale;
-                    }
-                } else {
+                for (int h = 0; h < 2; ++h) {
+                    float pv[2], dsv[2];
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) {
-                        const int col = c * 32 + i;
+                    for (int e = 0; e < 2; ++e) {
+                        const int col = 8 * i + c_in + e;
                         const int qi = q0 + col;
-                        float s2 = __uint_as_float(sr[i]) * p.scale_log2;
+                        float s2 = sacc[4 * i + 2 * h + e] * p.scale_log2;
                         float pr;
                         if (full_vis) {
                             pr = exp2f(s2 - lse2[col]);
                         } else if (MODE == MODE_PIVOT) {
-                            const bool vis = my_pos < bnd[col];
+                            const bool vis = my_pos[h] < bnd[col];
                             s2 = vis ? s2 + p.piv_bias_log2 : masked_val;
-                            pr = (kj < p.sk && qi < p.s) ? exp2f(s2 - lse2[col]) : 0.f;
+                            pr = (kj[h] < p.sk && qi < p.s) ? exp2f(s2 - lse2[col]) : 0.f;
                         } else {
-                            const bool vis = (MODE == MODE_BAND) ? (kj >= bnd[col] && kj <= qi)
-                                                                 : ((kj < p.sep_eff) || (kj <= qi));
+                            const bool vis = (MODE == MODE_BAND) ? (kj[h] >= bnd[col] && kj[h] <= qi)
+                                                                 : ((kj[h] < p.sep_eff) || (kj[h] <= qi));
                             if (!vis) s2 = masked_val;
-                            pr = (kj < p.s && qi < p.s) ? exp2f(s2 - lse2[col]) : 0.f;
+                            pr = (kj[h] < p.s && qi < p.s) ? exp2f(s2 - lse2[col]) : 0.f;
                         }
-                        float dp = __uint_as_float(dr[i]);
+                        float dp = dpacc[4 * i + 2 * h + e];
                         float pdrop = pr;
                         if (use_drop) {   // dP flows back through the keep mask; dV sees the dropped probabilities
-                            const bool keep = (kwc >> i) & 1u;
+                            const uint4 k4 = kw[h];
+                            const int wi = col >> 5;
+                            const uint32_t word = wi == 0 ? k4.x : (wi == 1 ? k4.y : (wi == 2 ? k4.z : k4.w));
+                            const bool keep = (word >> (col & 31)) & 1u;
                             dp = keep ? dp * p.drop_scale : 0.f;
                             pdrop = keep ? pr * p.drop_scale : 0.f;
                         }
-                        pv[i] = pdrop;
-                        dv[i] = pr * (dp - dlt[col]) * p.scale;
+                        pv[e] = pdrop;
+                        dsv[e] = pr * (dp - dlt[col]) * p.scale;
                     }
+                    ppk[2 * i + h] = pack_bf16x2(pv[0], pv[1]);
+                    dspk[2 * i + h] = pack_bf16x2(dsv[0], dsv[1]);
                 }
+            // dS^T -> shared memory (128B-swizzled, two 64-query sub-tiles) for the dQ product of both warpgroups
+            uint8_t* dbuf = sDST + buf * PT_BYTES;
 #pragma unroll
-                for (int g = 0; g < 4; ++g) {          // 4 chunks of 8 queries (16 bytes)
-                    uint4 a, d;
-                    a.x = pack_bf16x2(pv[g * 8 + 0], pv[g * 8 + 1]); a.y = pack_bf16x2(pv[g * 8 + 2], pv[g * 8 + 3]);
-                    a.z = pack_bf16x2(pv[g * 8 + 4], pv[g * 8 + 5]); a.w = pack_bf16x2(pv[g * 8 + 6], pv[g * 8 + 7]);
-                    d.x = pack_bf16x2(dv[g * 8 + 0], dv[g * 8 + 1]); d.y = pack_bf16x2(dv[g * 8 + 2], dv[g * 8 + 3]);
-                    d.z = pack_bf16x2(dv[g * 8 + 4], dv[g * 8 + 5]); d.w = pack_bf16x2(dv[g * 8 + 6], dv[g * 8 + 7]);
-                    const int chunk = c * 4 + g;           // 16-byte chunk index along the 128 queries
-                    const int sub = chunk >> 3, cc = chunk & 7;
-                    const int off = sub * (BLK * 128) + ((cc ^ (row & 7)) << 4);
-                    *reinterpret_cast<uint4*>(prow + off) = a;
-                    *reinterpret_cast<uint4*>(drow + off) = d;
+            for (int i = 0; i < BLK / 8; ++i)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int row = r_loc + 8 * h;
+                    const int sub = i >> 3, chunk = i & 7;
+                    *reinterpret_cast<uint32_t*>(dbuf + sub * (BLK * 128) + row * 128 + ((chunk ^ (row & 7)) << 4) +
+                                                 2 * c_in) = dspk[2 * i + h];
                 }
-            }
             fence_proxy_async_smem();
-            tc_fence_before();
-            mbar_arrive(pds_full);
-            // dQ tile of this (query block, key block) pair
-            mbar_wait(dq_full, t & 1);
-            tc_fence_after();
-            {
-                uint32_t r[HD / 2];                    // this thread's 32 of the row's 64 dims
-                tmem_ld_x32(lane_addr + TM_DQ + hf * (HD / 2), r);
-                tmem_ld_wait();
-                tc_fence_before();
-                mbar_arrive(dq_free);
-                const int qi = q0 + row;               // here `row` indexes the query (dQ tile rows are queries)
+            // dV += P^T dO,  dK += dS^T Q   (reduction over the 128 queries of this tile)
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < BLK / 16; ++k) {
+                uint32_t a[4];
+                frag_a(ppk, k, a);
+                wgmma_rs_n64<1>(dv, a, make_smem_desc_sw128(do_addr + k * 2048, BLK * 128, 1024), 1u);
+                frag_a(dspk, k, a);
+                wgmma_rs_n64<1>(dk, a, make_smem_desc_sw128(q_addr + k * 2048, BLK * 128, 1024), 1u);
+            }
+            wgmma_commit();
+            named_bar_sync(3, 256);                    // both halves of dS^T written
+            // dQ rows 64 half .. +63 of this query tile = dS K  (reduction over the 128 keys of this block)
+            float dq[HD / 2];
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < BLK / 16; ++k)
+                wgmma_ss_n64<1, 1>(dq, make_smem_desc_sw128(smem_u32(dbuf) + half * (BLK * 128) + k * 2048, BLK * 128, 1024),
+                                   make_smem_desc_sw128(k_addr + k * 2048, BLK * 128, 1024), k != 0 ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(dv);
+            fence_regs(dk);
+            fence_regs(dq);
+            if (lane == 0) mbar_arrive(&qdo_empty[stage]);
+            if (++stage == QDO_STAGES) { stage = 0; phase ^= 1; }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int qi = q0 + r_loc + 8 * h;     // dQ tile rows are queries
                 if (qi < p.s) {
-                    float* dst = p.dq_acc + ((size_t)batch * p.s + qi) * (p.heads * HD) + head * HD + hf * (HD / 2);
+                    float* dst = p.dq_acc + ((size_t)batch * p.s + qi) * (p.heads * HD) + head * HD;
 #pragma unroll
-                    for (int i = 0; i < HD / 2; i += 4)
-                        red_add_v4(dst + i, __uint_as_float(r[i]), __uint_as_float(r[i + 1]),
-                                   __uint_as_float(r[i + 2]), __uint_as_float(r[i + 3]));
-                }
-            }
-            if (++stage == QDO_STAGES) stage = 0;
-        }
-        // dK / dV of this key block: complete once the last tile's dV / dK MMAs retired (its pds_free commit)
-        mbar_wait(pds_free, (ntiles - 1) & 1);
-        tc_fence_after();
-        // (tcgen05.ld is warp-collective: every lane loads, only in-range rows store)
-        {
-            const int H3 = 3 * p.heads * HD;
-            const bool row_ok = kj < p.kv_rows;
-            __nv_bfloat16* base = p.dqkv + ((size_t)batch * p.kv_rows + (row_ok ? kj : 0)) * H3 + head * HD;
-            {
-                const int which = hf;                  // warps 2-5 store dK, warps 6-9 dV
-                uint32_t r[HD];
-                uint32_t (&r0)[32] = *reinterpret_cast<uint32_t(*)[32]>(&r[0]);
-                uint32_t (&r1)[32] = *reinterpret_cast<uint32_t(*)[32]>(&r[32]);
-                const uint32_t col = which == 0 ? TM_DK : TM_DV;
-                tmem_ld_x32(lane_addr + col, r0);
-                tmem_ld_x32(lane_addr + col + 32, r1);
-                tmem_ld_wait();
-                __nv_bfloat16* dst = base + (which == 0 ? 1 : 2) * (p.heads * HD);
-                if (row_ok) {
-#pragma unroll
-                for (int c = 0; c < HD / 8; ++c) {
-                    uint4 pk;
-                    pk.x = pack_bf16x2(__uint_as_float(r[c * 8 + 0]), __uint_as_float(r[c * 8 + 1]));
-                    pk.y = pack_bf16x2(__uint_as_float(r[c * 8 + 2]), __uint_as_float(r[c * 8 + 3]));
-                    pk.z = pack_bf16x2(__uint_as_float(r[c * 8 + 4]), __uint_as_float(r[c * 8 + 5]));
-                    pk.w = pack_bf16x2(__uint_as_float(r[c * 8 + 6]), __uint_as_float(r[c * 8 + 7]));
-                    *reinterpret_cast<uint4*>(dst + c * 8) = pk;
-                }
+                    for (int i = 0; i < HD / 8; ++i) red_add_v2(dst + 8 * i + c_in, dq[4 * i + 2 * h], dq[4 * i + 2 * h + 1]);
                 }
             }
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp_idx == 1) {
-        tc_fence_after();
-        tmem_dealloc<512>(tmem_base);
+        // dK / dV of this key block
+        const int H3 = 3 * p.heads * HD;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            if (kj[h] >= p.kv_rows) continue;
+            __nv_bfloat16* base = p.dqkv + ((size_t)batch * p.kv_rows + kj[h]) * H3 + head * HD;
+#pragma unroll
+            for (int i = 0; i < HD / 8; ++i) {
+                *reinterpret_cast<uint32_t*>(base + p.heads * HD + 8 * i + c_in) =
+                    pack_bf16x2(dk[4 * i + 2 * h], dk[4 * i + 2 * h + 1]);
+                *reinterpret_cast<uint32_t*>(base + 2 * p.heads * HD + 8 * i + c_in) =
+                    pack_bf16x2(dv[4 * i + 2 * h], dv[4 * i + 2 * h + 1]);
+            }
+        }
     }
 }
 

@@ -12,12 +12,12 @@
 // Q, K, V are read in place from the packed QKV GEMM output [b, s, 3h] (or a KV cache) through 3-D TMA
 // tensor maps; the context is written token-major [b, sq, h] — the layout the out-projection GEMM reads.
 //
-// One CTA per (128-query block, head, batch); 10 warps:
-//   warp 0     TMA producer (Q once; K/V tiles of 128 keys through a 3-stage ring)
-//   warp 1     tcgen05.mma issuer:  S = Q K^T (128x128x64) into TMEM;  O_j = P_j V_j (128x64x128) into TMEM
-//   warps 2-9  softmax: two threads per query row (64 keys / 32 output dims each); tcgen05.ld S, online max/sum, P
-//              (bf16) -> swizzled smem, then accumulate O_j from TMEM into registers with the running rescale
-// S and O are double-buffered in TMEM so S_{j+1} is computed while the softmax of tile j runs.
+// One CTA per (128-query block, head, batch); 3 warpgroups:
+//   warpgroup 0     TMA producer (one thread): Q once, K/V tiles of 128 keys through a 3-stage ring
+//   warpgroups 1-2  64 query rows each: S = Q K^T (wgmma m64n128k16, fp32 in registers), online softmax in registers
+//                   (the four threads of a quad share a pair of rows), P as bf16 registers straight into the A operand
+//                   of O += P V (m64n64k16).  The two warpgroups run independently, so the softmax of one overlaps
+//                   the MMAs of the other.
 #include "common.cuh"
 #include "host.h"
 #include "../../include/cogview_b200.h"
@@ -32,9 +32,8 @@ constexpr int KV_STAGES = 3;
 constexpr int Q_BYTES = BQ * HD * 2;        // 16 KB
 constexpr int K_BYTES = BKV * HD * 2;       // 16 KB
 constexpr int V_BYTES = BKV * HD * 2;       // 16 KB
-constexpr int P_BYTES = BQ * BKV * 2;       // 32 KB (two 128x64 K-major sub-tiles)
-constexpr int SMEM_BYTES = Q_BYTES + KV_STAGES * (K_BYTES + V_BYTES) + 2 * P_BYTES + 1024 + 256 + 1024 /*sPos*/ + 6 * BQ * 4 /*sX*/;
-constexpr int NUM_THREADS = 320;
+constexpr int SMEM_BYTES = Q_BYTES + KV_STAGES * (K_BYTES + V_BYTES) + 1024 + 256;
+constexpr int NUM_THREADS = 384;
 constexpr float LOG2E = 1.4426950408889634f;
 
 struct AttnParams {
@@ -76,19 +75,12 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* sQ = smem;
     uint8_t* sKV = sQ + Q_BYTES;                              // stage s: K at s*(K+V), V after it
-    uint8_t* sP = sKV + KV_STAGES * (K_BYTES + V_BYTES);      // 2 buffers
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sP + 2 * P_BYTES);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sKV + KV_STAGES * (K_BYTES + V_BYTES));
     uint64_t* q_full = bars;                 // [1]
     uint64_t* kv_full = bars + 1;            // [KV_STAGES]
-    uint64_t* kv_empty = kv_full + KV_STAGES;
-    uint64_t* s_full = kv_empty + KV_STAGES; // [2]
-    uint64_t* p_full = s_full + 2;           // [2]
-    uint64_t* o_full = p_full + 2;           // [2]
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(o_full + 2);
-    int* sPos = reinterpret_cast<int*>(bars + 32);           // [2][BKV] pivot positions of the current pivot tile
-    float* sX = reinterpret_cast<float*>(sPos + 2 * BKV);    // [2 tiles][2 halves][BQ] row maxima, [2][BQ] row sums
+    uint64_t* kv_empty = kv_full + KV_STAGES;// [KV_STAGES]: one arrive per consumer warp
 
-    const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
     // heaviest (last) query blocks first
     const int qb = gridDim.x - 1 - blockIdx.x;
     const int head = blockIdx.y, batch = blockIdx.z;
@@ -109,29 +101,24 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         nkb = nband + npt;
     }
 
-    if (warp_idx == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmQ);
         tma_prefetch_desc(&tmK);
         tma_prefetch_desc(&tmV);
         mbar_init(q_full, 1);
-        for (int i = 0; i < KV_STAGES; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&s_full[i], 1); mbar_init(&p_full[i], 256); mbar_init(&o_full[i], 1); }
+        for (int i = 0; i < KV_STAGES; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 8); }
         fence_barrier_init();
     }
-    if (warp_idx == 1) tmem_alloc<512>(tmem_ptr);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
-    const uint32_t TM_S = 0, TM_O = 256;     // column offsets: S0, S1 (128 each); O0, O1 (64 each)
 
-    if (warp_idx == 0) {
-        if (lane == 0) {
+    if (wg == 0) {
+        setmaxnreg_dec<40>();
+        if (tid == 0) {
             mbar_expect_tx(q_full, Q_BYTES);
             tma_load_3d(sQ, &tmQ, q_full, head * HD, q0, batch);
             int stage = 0; uint32_t phase = 0;
             for (int j = 0; j < nkb; ++j) {
-                mbar_wait(&kv_empty[stage], phase ^ 1);
+                mbar_wait<false>(&kv_empty[stage], phase ^ 1);
                 uint8_t* sK = sKV + stage * (K_BYTES + V_BYTES);
                 mbar_expect_tx(&kv_full[stage], K_BYTES + V_BYTES);
                 if (SPARSE && j >= nband) {
@@ -144,219 +131,162 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
                 if (++stage == KV_STAGES) { stage = 0; phase ^= 1; }
             }
         }
-    } else if (warp_idx == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc_s = make_idesc_bf16(BQ, BKV, 0, 0);  // Q K-major, K K-major
-            constexpr uint32_t idesc_o = make_idesc_bf16(BQ, HD, 0, 1);   // P K-major, V MN-major
-            const uint32_t q_addr = smem_u32(sQ);
-            auto issue_s = [&](int j, int stage) {
-                const uint32_t k_addr = smem_u32(sKV + stage * (K_BYTES + V_BYTES));
-#pragma unroll
-                for (int k = 0; k < HD / 16; ++k) {
-                    umma_f16(tmem_base + TM_S + (j & 1) * BKV, make_smem_desc_sw128(q_addr + k * 32, 0, 1024),
-                             make_smem_desc_sw128(k_addr + k * 32, 0, 1024), idesc_s, k != 0);
-                }
-                umma_commit(&s_full[j & 1]);
-            };
-            mbar_wait(q_full, 0);
-            int ld_stage = 0; uint32_t ld_phase = 0;   // stage/phase of the next tile whose S is issued
-            mbar_wait(&kv_full[0], 0);
-            tc_fence_after();
-            issue_s(0, 0);
-            ld_stage = 1 % KV_STAGES;
-            int pv_stage = 0;
-            for (int j = 0; j < nkb; ++j) {
-                if (j + 1 < nkb) {
-                    mbar_wait(&kv_full[ld_stage], ld_phase);
-                    tc_fence_after();
-                    issue_s(j + 1, ld_stage);
-                    if (++ld_stage == KV_STAGES) { ld_stage = 0; ld_phase ^= 1; }
-                }
-                mbar_wait(&p_full[j & 1], (j >> 1) & 1);
-                tc_fence_after();
-                const uint32_t p_addr = smem_u32(sP + (j & 1) * P_BYTES);
-                const uint32_t v_addr = smem_u32(sKV + pv_stage * (K_BYTES + V_BYTES) + K_BYTES);
-#pragma unroll
-                for (int k = 0; k < BKV / 16; ++k) {
-                    const uint32_t pa = p_addr + (k >> 2) * (BQ * 128) + (k & 3) * 32;
-                    umma_f16(tmem_base + TM_O + (j & 1) * HD, make_smem_desc_sw128(pa, 0, 1024),
-                             make_smem_desc_sw128(v_addr + k * (16 * 128), BKV * 128, 1024), idesc_o, k != 0);
-                }
-                umma_commit(&o_full[j & 1]);
-                umma_commit(&kv_empty[pv_stage]);
-                if (++pv_stage == KV_STAGES) pv_stage = 0;
-            }
-        }
     } else {
-        // ------------------------------ softmax / output warps ------------------------------
-        // 8 warps: warp w works on TMEM lane quadrant w % 4 (rows 32 (w % 4) .. +31, one row per lane) and on HALF of the
-        // row: warps 2-5 the first 64 keys of every tile and output dims 0-31, warps 6-9 the other half.  Two threads
-        // per row halve the serial exp2 / pack / rescale chain of a tile and give every scheduler two softmax warps to
-        // overlap (one warp per scheduler ran at 8 % tensor-pipe utilisation, profiles/r01_ncu_full_attention_summary);
-        // the only exchange per tile is the row maximum (shared memory + a 64-thread named barrier per quadrant).
-        const int q = warp_idx & 3;
-        const int hf = (warp_idx - 2) >> 2;
-        const int row = q * 32 + lane;
-        const int qi = q0 + row;                       // query index within the sequence
-        const uint32_t lane_addr = tmem_base + (uint32_t(q * 32) << 16);
-        const int causal_lim = qi + p.off;             // last causally visible key
-        const int bs_row = SPARSE ? band_start(qi, p.sp_w, p.sp_times) : 0;
-        constexpr int HK = BKV / 2, HO = HD / 2;       // keys / output dims per thread
-        float m = -INFINITY, l = 0.f, alpha_prev = 0.f;
-        float o[HO];
+        // ------------------------------ MMA + softmax warpgroups ------------------------------
+        // Fragment layout (common.cuh): this thread holds rows r_loc and r_loc + 8 of the block, and of every
+        // 8-column group the two columns c_in, c_in + 1.  Row statistics are reduced over the 4 lanes of a quad.
+        setmaxnreg_inc<232>();
+        const int half = wg - 1, warp = tid >> 5, lane = tid & 31;
+        const int r_loc = 64 * half + 16 * warp + (lane >> 2);
+        const int c_in = 2 * (lane & 3);
+        int qi[2], causal_lim[2], bs_row[2];
 #pragma unroll
-        for (int i = 0; i < HO; ++i) o[i] = 0.f;
+        for (int h = 0; h < 2; ++h) {
+            qi[h] = q0 + r_loc + 8 * h;                    // query index within the sequence
+            causal_lim[h] = qi[h] + p.off;                 // last causally visible key
+            bs_row[h] = SPARSE ? band_start(qi[h], p.sp_w, p.sp_times) : 0;
+        }
+        float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+        float o[HD / 2];
+#pragma unroll
+        for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
         const float masked_val = -10000.0f * LOG2E;
-        const uint4* keep_row = nullptr;
-        uint4 pre_keep = make_uint4(0u, 0u, 0u, 0u);
+        const uint4* keep_row[2] = {nullptr, nullptr};
         if (DROPOUT) {
             const size_t region = (size_t)p.b * p.heads * p.nkb_all * p.nqb_all * (BQ * 4);   // words per region
-            keep_row = reinterpret_cast<const uint4*>(p.drop_mask + region) +
-                       (((size_t)batch * p.heads + head) * p.nqb_all * BQ + qi) * p.nkb_all;
-            pre_keep = keep_row[0];
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+                keep_row[h] = reinterpret_cast<const uint4*>(p.drop_mask + region) +
+                              (((size_t)batch * p.heads + head) * p.nqb_all * BQ + qi[h]) * p.nkb_all;
         }
-
+        const uint32_t q_addr = smem_u32(sQ) + half * (64 * 128);
+        mbar_wait<false>(q_full, 0);
+        int stage = 0; uint32_t phase = 0;
         for (int j = 0; j < nkb; ++j) {
-            uint32_t kw0 = 0u, kw1 = 0u;                // keep bits of this row over this thread's 64 keys
-            if (DROPOUT) {
-                kw0 = hf ? pre_keep.z : pre_keep.x;
-                kw1 = hf ? pre_keep.w : pre_keep.y;
-                if (j + 1 < nkb) pre_keep = keep_row[j + 1];
-            }
+            uint4 kw[2] = {make_uint4(0u, 0u, 0u, 0u), make_uint4(0u, 0u, 0u, 0u)};
+            if (DROPOUT) { kw[0] = keep_row[0][j]; kw[1] = keep_row[1][j]; }
             const bool piv_tile = SPARSE && j >= nband;
-            if (piv_tile) {                             // positions of this tile's 128 gathered keys -> shared memory
-                if (hf == 0) {
-                    const int pj = (j - nband) * BKV + row;
-                    sPos[(j & 1) * BKV + row] = pj < p.n_piv ? p.piv_pos[(size_t)batch * p.n_piv + pj] : 0x7fffffff;
-                }
-                named_bar_sync(2, 256);
-            }
-            mbar_wait(&s_full[j & 1], (j >> 1) & 1);
-            tc_fence_after();
             const int k0 = SPARSE ? (piv_tile ? (j - nband) * BKV : (jb0 + j) * BKV) : j * BKV;
-            const int kb = k0 + hf * HK;                // first key of this thread's half
-            // does this tile need per-element masking for this row?
-            const bool full_vis = SPARSE ? (!piv_tile && k0 >= bs_row && k0 + BKV - 1 <= qi && k0 + BKV <= p.sk)
-                                         : (k0 + BKV <= p.sk) && ((k0 + BKV <= p.sep_eff) || (k0 + BKV - 1 <= causal_lim));
-            float s[HK];
+            mbar_wait<false>(&kv_full[stage], phase);
+            const uint32_t k_addr = smem_u32(sKV + stage * (K_BYTES + V_BYTES));
+            const uint32_t v_addr = k_addr + K_BYTES;
+            float s[BKV / 2];
+            wgmma_fence();
 #pragma unroll
-            for (int c = 0; c < HK / 32; ++c) {
-                uint32_t (&r)[32] = *reinterpret_cast<uint32_t(*)[32]>(&s[c * 32]);
-                tmem_ld_x32(lane_addr + TM_S + (j & 1) * BKV + hf * HK + c * 32, r);
+            for (int k = 0; k < HD / 16; ++k)
+                wgmma_ss_n128<0, 0>(s, make_smem_desc_sw128(q_addr + k * 32, 0, 1024),
+                                    make_smem_desc_sw128(k_addr + k * 32, 0, 1024), k != 0 ? 1u : 0u);
+            wgmma_commit();
+            int pos[SPARSE ? BKV / 4 : 1];              // positions of this thread's 32 gathered keys (pivot tiles)
+            if (piv_tile) {
+#pragma unroll
+                for (int i = 0; i < BKV / 8; ++i)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int pj = k0 + 8 * i + c_in + e;
+                        pos[2 * i + e] = pj < p.n_piv ? p.piv_pos[(size_t)batch * p.n_piv + pj] : 0x7fffffff;
+                    }
             }
-            tmem_ld_wait();
-            float mx = -INFINITY;
-            if (full_vis) {
+            wgmma_wait<0>();
+            fence_regs(s);
+            float alpha[2];
 #pragma unroll
-                for (int i = 0; i < HK; ++i) { s[i] *= p.scale_log2; mx = fmaxf(mx, s[i]); }
-            } else if (piv_tile) {
-                const int* pos = sPos + (j & 1) * BKV + hf * HK;
+            for (int h = 0; h < 2; ++h) {
+                // does this tile need per-element masking for this row?
+                const bool full_vis = SPARSE ? (!piv_tile && k0 >= bs_row[h] && k0 + BKV - 1 <= qi[h] && k0 + BKV <= p.sk)
+                                             : (k0 + BKV <= p.sk) && ((k0 + BKV <= p.sep_eff) || (k0 + BKV - 1 <= causal_lim[h]));
+                float mx = -INFINITY;
 #pragma unroll
-                for (int i = 0; i < HK; ++i) {
-                    const int pp = pos[i];
-                    float v = pp < bs_row ? s[i] * p.scale_log2 + p.piv_bias_log2 : masked_val;
-                    if (pp == 0x7fffffff) v = -INFINITY;   // beyond the pivot list
-                    s[i] = v;
-                    mx = fmaxf(mx, v);
+                for (int i = 0; i < BKV / 8; ++i)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        float& x = s[4 * i + 2 * h + e];
+                        const int kj = k0 + 8 * i + c_in + e;
+                        float v;
+                        if (full_vis) {
+                            v = x * p.scale_log2;
+                        } else if (piv_tile) {
+                            const int pp = pos[SPARSE ? 2 * i + e : 0];
+                            v = pp < bs_row[h] ? x * p.scale_log2 + p.piv_bias_log2 : masked_val;
+                            if (pp == 0x7fffffff) v = -INFINITY;   // beyond the pivot list
+                        } else {
+                            const bool vis = SPARSE ? (kj >= bs_row[h] && kj <= qi[h])
+                                                    : ((kj < p.sep_eff) || (kj <= causal_lim[h]));
+                            v = vis ? x * p.scale_log2 : masked_val;
+                            if (kj >= p.sk) v = -INFINITY;     // key does not exist
+                        }
+                        x = v;
+                        mx = fmaxf(mx, v);
+                    }
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+                mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+                mx = fmaxf(mx, m[h]);
+                alpha[h] = exp2f(m[h] - mx);                // m = -inf on the first tile -> 0
+                m[h] = mx;
+            }
+            uint32_t pk[BKV / 4];                           // bf16 pairs of P in the A-fragment order
+            float psum[2] = {0.f, 0.f};
+#pragma unroll
+            for (int i = 0; i < BKV / 8; ++i)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    float e0 = exp2f(s[4 * i + 2 * h] - m[h]), e1 = exp2f(s[4 * i + 2 * h + 1] - m[h]);
+                    uint32_t w = pack_bf16x2(e0, e1);
+                    // the row sum uses the bf16-rounded probabilities that the PV MMA will see
+                    const __nv_bfloat162 pb = *reinterpret_cast<const __nv_bfloat162*>(&w);
+                    psum[h] += __low2float(pb) + __high2float(pb);
+                    if (DROPOUT) {   // dropout acts on the normalised probabilities: the row sum stays undropped; the
+                                     // 1/(1-p) scale is applied once to the output row at the end
+                        const uint4 k4 = kw[h];
+                        const uint32_t word = (i >> 2) == 0 ? k4.x : ((i >> 2) == 1 ? k4.y : ((i >> 2) == 2 ? k4.z : k4.w));
+                        const int bit = 8 * (i & 3) + c_in;
+                        w = pack_bf16x2(((word >> bit) & 1u) ? e0 : 0.f, ((word >> (bit + 1)) & 1u) ? e1 : 0.f);
+                    }
+                    pk[2 * i + h] = w;
                 }
-            } else {
 #pragma unroll
-                for (int i = 0; i < HK; ++i) {
-                    const int kj = kb + i;
-                    const bool vis = SPARSE ? (kj >= bs_row && kj <= qi) : ((kj < p.sep_eff) || (kj <= causal_lim));
-                    float v = vis ? s[i] * p.scale_log2 : masked_val;
-                    if (kj >= p.sk) v = -INFINITY;     // key does not exist
-                    s[i] = v;
-                    mx = fmaxf(mx, v);
-                }
+            for (int h = 0; h < 2; ++h) l[h] = l[h] * alpha[h] + psum[h];   // this thread's share of the row sum
+#pragma unroll
+            for (int i = 0; i < HD / 8; ++i) {
+                o[4 * i + 0] *= alpha[0]; o[4 * i + 1] *= alpha[0];
+                o[4 * i + 2] *= alpha[1]; o[4 * i + 3] *= alpha[1];
             }
-            // row maximum over both halves
-            sX[((j & 1) * 2 + hf) * BQ + row] = mx;
-            named_bar_sync(3 + q, 64);
-            mx = fmaxf(fmaxf(mx, sX[((j & 1) * 2 + (hf ^ 1)) * BQ + row]), m);
-            const float alpha = exp2f(m - mx);          // m = -inf on the first tile -> 0
-            m = mx;
-            float psum = 0.f;
-            uint8_t* prow = sP + (j & 1) * P_BYTES + hf * (BQ * 128) + row * 128;   // this half = one 64-key sub-tile
+            fence_regs(o);
+            wgmma_fence();
 #pragma unroll
-            for (int c = 0; c < HK / 8; ++c) {          // 8 chunks of 8 keys (16 bytes)
-                float e[8];
-#pragma unroll
-                for (int t = 0; t < 8; ++t) e[t] = exp2f(s[c * 8 + t] - mx);
-                uint4 pk;
-                pk.x = pack_bf16x2(e[0], e[1]); pk.y = pack_bf16x2(e[2], e[3]);
-                pk.z = pack_bf16x2(e[4], e[5]); pk.w = pack_bf16x2(e[6], e[7]);
-                // the row sum uses the bf16-rounded probabilities that the PV MMA will see
-                const __nv_bfloat162* pb = reinterpret_cast<const __nv_bfloat162*>(&pk);
-#pragma unroll
-                for (int t = 0; t < 4; ++t) psum += __low2float(pb[t]) + __high2float(pb[t]);
-                if (DROPOUT) {   // dropout acts on the normalised probabilities: the row sum stays undropped; the
-                                 // 1/(1-p) scale is applied once to the output row at the end
-                    const uint32_t w = (c >> 2) == 0 ? kw0 : kw1;
-#pragma unroll
-                    for (int t = 0; t < 8; ++t) e[t] = ((w >> ((c & 3) * 8 + t)) & 1u) ? e[t] : 0.f;
-                    pk.x = pack_bf16x2(e[0], e[1]); pk.y = pack_bf16x2(e[2], e[3]);
-                    pk.z = pack_bf16x2(e[4], e[5]); pk.w = pack_bf16x2(e[6], e[7]);
-                }
-                *reinterpret_cast<uint4*>(prow + ((c ^ (row & 7)) << 4)) = pk;
+            for (int kk = 0; kk < BKV / 16; ++kk) {
+                uint32_t a[4];
+                frag_a(pk, kk, a);
+                wgmma_rs_n64<1>(o, a, make_smem_desc_sw128(v_addr + kk * (16 * 128), BKV * 128, 1024), 1u);
             }
-            l = l * alpha + psum;                       // this half's share of the row sum
-            fence_proxy_async_smem();
-            tc_fence_before();
-            mbar_arrive(&p_full[j & 1]);
-            if (j > 0) {
-                mbar_wait(&o_full[(j - 1) & 1], ((j - 1) >> 1) & 1);
-                tc_fence_after();
-                uint32_t r[HO];
-                tmem_ld_x32(lane_addr + TM_O + ((j - 1) & 1) * HD + hf * HO, r);
-                tmem_ld_wait();
-#pragma unroll
-                for (int i = 0; i < HO; ++i) o[i] = o[i] * alpha_prev + __uint_as_float(r[i]);
-            }
-            alpha_prev = alpha;
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(o);
+            if (lane == 0) mbar_arrive(&kv_empty[stage]);
+            if (++stage == KV_STAGES) { stage = 0; phase ^= 1; }
         }
-        {
-            const int j = nkb - 1;
-            mbar_wait(&o_full[j & 1], (j >> 1) & 1);
-            tc_fence_after();
-            uint32_t r[HO];
-            tmem_ld_x32(lane_addr + TM_O + (j & 1) * HD + hf * HO, r);
-            tmem_ld_wait();
 #pragma unroll
-            for (int i = 0; i < HO; ++i) o[i] = o[i] * alpha_prev + __uint_as_float(r[i]);
-        }
-        // total row sum = the two halves' shares
-        sX[(4 + hf) * BQ + row] = l;
-        named_bar_sync(3 + q, 64);
-        l += sX[(4 + (hf ^ 1)) * BQ + row];
-        if (qi < p.sq) {
-            const float inv_l = (DROPOUT ? p.drop.scale : 1.0f) / l;
-            __nv_bfloat16* orow = p.out + (size_t)batch * p.bso + (size_t)qi * p.ldo + head * HD + hf * HO;
+        for (int h = 0; h < 2; ++h) {
+            float lt = l[h];
+            lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+            lt += __shfl_xor_sync(0xffffffffu, lt, 2);
+            if (qi[h] < p.sq) {
+                const float inv_l = (DROPOUT ? p.drop.scale : 1.0f) / lt;
+                __nv_bfloat16* orow = p.out + (size_t)batch * p.bso + (size_t)qi[h] * p.ldo + head * HD;
 #pragma unroll
-            for (int c = 0; c < HO / 8; ++c) {
-                uint4 pk;
-                pk.x = pack_bf16x2(o[c * 8 + 0] * inv_l, o[c * 8 + 1] * inv_l);
-                pk.y = pack_bf16x2(o[c * 8 + 2] * inv_l, o[c * 8 + 3] * inv_l);
-                pk.z = pack_bf16x2(o[c * 8 + 4] * inv_l, o[c * 8 + 5] * inv_l);
-                pk.w = pack_bf16x2(o[c * 8 + 6] * inv_l, o[c * 8 + 7] * inv_l);
-                *reinterpret_cast<uint4*>(orow + c * 8) = pk;
+                for (int i = 0; i < HD / 8; ++i)
+                    *reinterpret_cast<uint32_t*>(orow + 8 * i + c_in) =
+                        pack_bf16x2(o[4 * i + 2 * h] * inv_l, o[4 * i + 2 * h + 1] * inv_l);
+                if ((lane & 3) == 0 && p.lse != nullptr)
+                    p.lse[((size_t)batch * p.heads + head) * p.sq + qi[h]] = m[h] * 0.6931471805599453f + logf(lt);
             }
-            if (hf == 0 && p.lse != nullptr)
-                p.lse[((size_t)batch * p.heads + head) * p.sq + qi] = m * 0.6931471805599453f + logf(l);
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp_idx == 1) {
-        tc_fence_after();
-        tmem_dealloc<512>(tmem_base);
     }
 }
 
 // Keep decisions of the attention-probability dropout for every (query, key) pair of the visible tiles, generated
 // ahead of the attention kernel at full occupancy (inside the attention kernel the same work sits on the softmax
-// warps' critical path: measured +200 us per call at the 4B shape).  One thread per (query row, key tile): a
+// warps' critical path).  One thread per (query row, key tile): a
 // Philox4x32-10 call seeds four 32-step LCG streams, keep iff state >= p * 2^32.  Writes both layouts (AttnParams).
 __global__ void __launch_bounds__(128, 4)
 attn_dropout_mask_kernel(const AttnParams p) {

@@ -1,5 +1,5 @@
-// Shared device-side primitives for the sm_100a kernels: mbarrier, TMA, tcgen05 / TMEM,
-// UMMA descriptors, warp reductions.  Everything is inline PTX; no CUTLASS/CuTe dependency.
+// Shared device-side primitives for the sm_90a kernels: mbarrier, TMA, wgmma and its shared-memory
+// descriptors, warp reductions.  Everything is inline PTX; no CUTLASS/CuTe dependency.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -140,6 +140,9 @@ __device__ __forceinline__ uint64_t global_timer_ns() {
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
     return t;
 }
+// TRACE = false: no printf on the timeout path (a function call there would make ptxas serialise the wgmma of a
+// warpgroup that waits with MMAs still in flight)
+template <bool TRACE = true>
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     uint32_t addr = smem_u32(bar);
     uint32_t done = 0;
@@ -160,8 +163,9 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
             const uint64_t now = global_timer_ns();
             if (t0 == 0) t0 = now;
             else if (now - t0 > CV_WAIT_TIMEOUT_NS) {
-                printf("cogview_b200: mbarrier wait timed out (block %d,%d,%d thread %d, smem 0x%x, parity %u)\n",
-                       blockIdx.x, blockIdx.y, blockIdx.z, threadIdx.x, addr, parity);
+                if (TRACE)
+                    printf("cogview_b200: mbarrier wait timed out (block %d,%d,%d thread %d, smem 0x%x, parity %u)\n",
+                           blockIdx.x, blockIdx.y, blockIdx.z, threadIdx.x, addr, parity);
                 __trap();
             }
         }
@@ -221,98 +225,59 @@ template <int N>
 __device__ __forceinline__ void tma_store_wait_all() {
     asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
-// make generic-proxy smem writes visible to the async proxy (TMA store / tcgen05.mma operand reads)
+// make generic-proxy smem writes visible to the async proxy (TMA store / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// wgmma (warpgroup MMA, sm_90a): accumulators live in the registers of the 128 threads of a warpgroup
 // ----------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// make the warpgroup's register / shared-memory writes visible to the wgmma that follow
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// wait until at most N committed wgmma groups of this warpgroup are still in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keep the accumulator registers ordered around the asynchronous wgmma
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// move the register budget between the producer warpgroup and the MMA warpgroups
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
-// whole warp; writes the allocated TMEM base address to *dst (shared memory)
-template <uint32_t NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst)), "n"(NCOLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// Accumulator fragment of an m64nN wgmma, thread t of the warpgroup (warp w = t / 32, lane l):
+//   d[4i + e]     row 16w + l/4,      column 8i + 2(l%4) + e     (e = 0, 1)
+//   d[4i + 2 + e] row 16w + l/4 + 8,  same column
+// The A-from-registers fragment of a k16 slice uses the same positions: the bf16 pairs of d[8k .. 8k+7] of an
+// accumulator are the A operand for k-columns 16k .. 16k+15 (frag_a below).
+__device__ __forceinline__ void frag_a(const uint32_t* packed, int k, uint32_t (&a)[4]) {
+    a[0] = packed[4 * k]; a[1] = packed[4 * k + 1]; a[2] = packed[4 * k + 2]; a[3] = packed[4 * k + 3];
 }
-template <uint32_t NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; single thread issues.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                         uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-
-// TMEM -> registers: lane = 32*(warp%4) + threadIdx%32, N consecutive 32-bit columns
-__device__ __forceinline__ void tmem_ld_x32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------------------------
-// UMMA descriptors (bit layout: PTX ISA "tcgen05 shared memory descriptor" / "instruction descriptor")
-// ----------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, 128-byte swizzle.
+// wgmma shared-memory matrix descriptor (PTX ISA "Matrix Descriptor Format"), 128-byte swizzle:
 //   bits [0,14)  start address >> 4
 //   bits [16,30) leading-dimension byte offset >> 4
 //   bits [32,46) stride-dimension byte offset >> 4
-//   bits [46,48) descriptor version = 1 (Blackwell)
-//   bits [61,64) layout type: 2 = SWIZZLE_128B
+//   bits [62,64) layout type: 1 = SWIZZLE_128B
 // K-major operand (rows = M or N index, 128 bytes of K per row): 8-row groups SBO apart; LBO unused.
 // MN-major operand (rows = K index, 128 bytes of M/N per row): 8-row K groups SBO apart, 64-element
-// M/N chunks LBO apart.
+// M/N chunks LBO apart.  Every tile here starts 1024-byte aligned, so the base-offset field stays 0; stepping
+// along K inside a swizzled row is done by advancing the start address (32 bytes per k16 step, K-major).
+// ----------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     uint64_t d = 0;
     d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
     d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
     d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(2) << 61;
+    d |= static_cast<uint64_t>(1) << 62;
     return d;
 }
 
-// Instruction descriptor for kind::f16 with BF16 inputs and FP32 accumulation.
-//   [4,6) D format: 1 = F32;  [7,10) A format: 1 = BF16;  [10,13) B format: 1 = BF16
-//   bit 15 A major (0 = K, 1 = MN);  bit 16 B major;  [17,23) N >> 3;  [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t M, uint32_t N, uint32_t a_mn_major,
-                                                       uint32_t b_mn_major) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((N >> 3) << 17) |
-           ((M >> 4) << 24);
-}
-
 }  // namespace cv
+
+#include "wgmma.cuh"

@@ -1,4 +1,4 @@
-// VQ-VAE convolutions as im2col-free implicit GEMMs on tcgen05 (NHWC bf16 activations).
+// VQ-VAE convolutions as im2col-free implicit GEMMs on wgmma (NHWC bf16 activations).
 //
 //   cv_conv2d_k4s2           nn.Conv2d(Cin, Cout, 4, stride=2, padding=1)          encoder, /root/reference/vqvae/vqvae_zc.py:121-129
 //   cv_conv_transpose2d_k4s2 nn.ConvTranspose2d(Cin, Cout, 4, stride=2, padding=1) decoder, vqvae/vqvae_zc.py:172-191
@@ -8,8 +8,8 @@
 // strided convolution (elementStrides), out-of-bounds coordinates zero-filled by TMA (that IS the padding) — so
 // no im2col buffer is ever materialised.  Weights are pre-packed [tap][Cout][Cin] (K-major B tiles).
 // The transposed convolution is computed as its 4 sub-pixel phases (each a 2x2-tap stride-1 convolution on the
-// input grid); a phase's output tile is scattered to (2a+py, 2b+px) with one 5-D TMA store.
-// Pipeline / warp roles / TMEM double-buffering are those of gemm.cu; epilogue = bias (+ReLU) -> bf16 -> TMA store.
+// input grid); a phase's output pixels are scattered to (2a+py, 2b+px).
+// Pipeline and warpgroup roles are those of gemm.cu; epilogue = bias (+ReLU) -> bf16 -> global stores.
 #include "common.cuh"
 #include "host.h"
 #include "../../include/cogview_b200.h"
@@ -19,8 +19,7 @@ using namespace cv;
 
 constexpr int BM = 128;
 constexpr int BK = 64;
-constexpr int NUM_THREADS = 192;
-constexpr int EPI_BYTES = 128 * 128;
+constexpr int NUM_THREADS = 384;
 
 template <int BN>
 struct Cfg {
@@ -28,7 +27,7 @@ struct Cfg {
     static constexpr int B_BYTES = BN * BK * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
     static constexpr int STAGES = (BN == 256) ? 4 : 6;
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 2 * EPI_BYTES + 1024 + 256;
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
 };
 
 struct ConvParams {
@@ -40,47 +39,45 @@ struct ConvParams {
     int py, px;          // transposed conv: output phase
     const __nv_bfloat16* bias;
     int relu;
+    __nv_bfloat16* y;    // NHWC output
 };
+
+template <int N>
+__device__ __forceinline__ void conv_mma(float* acc, uint64_t da, uint64_t db, uint32_t sc) {
+    if constexpr (N == 256) wgmma_ss_n256<0, 0>(*reinterpret_cast<float(*)[128]>(acc), da, db, sc);
+    else wgmma_ss_n128<0, 0>(*reinterpret_cast<float(*)[64]>(acc), da, db, sc);
+}
 
 // MODE 1: conv k4 s2 p1.  MODE 2: one phase of convT k4 s2 p1.
 template <int BN, int MODE>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-            const __grid_constant__ CUtensorMap tmC, const ConvParams p) {
+conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const ConvParams p) {
     using C = Cfg<BN>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* epi_buf = smem + C::STAGES * C::STAGE_BYTES;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(epi_buf + 2 * EPI_BYTES);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);
     uint64_t* full_bar = bars;
-    uint64_t* empty_bar = bars + C::STAGES;
-    uint64_t* tmem_full = bars + 2 * C::STAGES;
-    uint64_t* tmem_empty = bars + 2 * C::STAGES + 2;
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * C::STAGES + 4);
+    uint64_t* empty_bar = bars + C::STAGES;          // one arrive per consumer warp
 
-    const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
     const int num_tiles = p.num_m_tiles * p.num_n_blocks;
     const int num_k_blocks = p.ntaps * p.kc_blocks;
 
-    if (warp_idx == 0 && lane == 0) {
-        tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmB); tma_prefetch_desc(&tmC);
-        for (int i = 0; i < C::STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(&tmem_full[i], 1); mbar_init(&tmem_empty[i], 128); }
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmB);
+        for (int i = 0; i < C::STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 8); }
         fence_barrier_init();
     }
-    if (warp_idx == 1) tmem_alloc<2 * BN>(tmem_ptr);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
 
     auto tile_origin = [&](int mt, int& b0, int& y0) {
         if (p.tiles_per_image >= 1) { b0 = mt / p.tiles_per_image; y0 = (mt % p.tiles_per_image) * p.TH; }
         else { b0 = mt * p.NB; y0 = 0; }
     };
 
-    if (warp_idx == 0) {
-        if (lane == 0) {
+    if (wg == 0) {
+        setmaxnreg_dec<40>();
+        if (tid == 0) {
             int stage = 0; uint32_t phase = 0;
             for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
                 const int mt = tile % p.num_m_tiles;
@@ -106,7 +103,7 @@ conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                         ay = y0 + dy;
                         wtap = ky * 4 + kx;
                     }
-                    mbar_wait(&empty_bar[stage], phase ^ 1);
+                    mbar_wait<false>(&empty_bar[stage], phase ^ 1);
                     uint8_t* sA = smem + stage * C::STAGE_BYTES;
                     mbar_expect_tx(&full_bar[stage], C::STAGE_BYTES);
                     tma_load_4d(sA, &tmA, &full_bar[stage], kc * BK, ax, ay, b0);
@@ -115,105 +112,72 @@ conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                 }
             }
         }
-    } else if (warp_idx == 1) {
-        if (lane == 0) {
-            constexpr uint32_t idesc = make_idesc_bf16(BM, BN, 0, 0);
-            int stage = 0; uint32_t phase = 0; int it = 0;
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-                const int as = it & 1;
-                const uint32_t aphase = (it >> 1) & 1;
-                mbar_wait(&tmem_empty[as], aphase ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + as * BN;
-                for (int kb = 0; kb < num_k_blocks; ++kb) {
-                    mbar_wait(&full_bar[stage], phase);
-                    tc_fence_after();
-                    const uint32_t a_addr = smem_u32(smem + stage * C::STAGE_BYTES);
-                    const uint32_t b_addr = a_addr + C::A_BYTES;
-#pragma unroll
-                    for (int k = 0; k < BK / 16; ++k)
-                        umma_f16(d_tmem, make_smem_desc_sw128(a_addr + k * 32, 0, 1024),
-                                 make_smem_desc_sw128(b_addr + k * 32, 0, 1024), idesc, (kb | k) != 0 ? 1u : 0u);
-                    umma_commit(&empty_bar[stage]);
-                    if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-                }
-                umma_commit(&tmem_full[as]);
-            }
-        }
     } else {
-        const int q = warp_idx & 3;
-        const int row = q * 32 + lane;
-        const int epi_tid = threadIdx.x - 64;
-        constexpr int NCHUNK = BN / 64;
-        int it = 0;
-        uint32_t buf_sel = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
+        setmaxnreg_inc<232>();
+        const int half = wg - 1;
+        const int warp = tid >> 5, lane = tid & 31;
+        const int r_in = 64 * half + 16 * warp + (lane >> 2);   // this thread's pixels r_in, r_in + 8 of the tile
+        const int c_in = 2 * (lane & 3);
+        int stage = 0; uint32_t phase = 0;
+        float acc[BN / 2];
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
             const int mt = tile % p.num_m_tiles;
             const int n0 = (tile / p.num_m_tiles) * BN;
+            int prev = -1;
+            for (int kb = 0; kb < num_k_blocks; ++kb) {
+                mbar_wait<false>(&full_bar[stage], phase);
+                const uint32_t a_addr = smem_u32(smem + stage * C::STAGE_BYTES) + half * (64 * 128);
+                const uint32_t b_addr = smem_u32(smem + stage * C::STAGE_BYTES + C::A_BYTES);
+                fence_regs(acc);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / 16; ++k)
+                    conv_mma<BN>(acc, make_smem_desc_sw128(a_addr + k * 32, 0, 1024),
+                                 make_smem_desc_sw128(b_addr + k * 32, 0, 1024), (kb | k) != 0 ? 1u : 0u);
+                wgmma_commit();
+                wgmma_wait<1>();
+                if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+                prev = stage;
+                if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+            }
+            wgmma_wait<0>();
+            fence_regs(acc);
+            if (lane == 0) mbar_arrive(&empty_bar[prev]);
             int b0, y0;
             tile_origin(mt, b0, y0);
-            const int as = it & 1;
-            const uint32_t aphase = (it >> 1) & 1;
-            mbar_wait(&tmem_full[as], aphase);
-            tc_fence_after();
-#pragma unroll 1
-            for (int c = 0; c < NCHUNK; ++c) {
-                const uint32_t taddr = tmem_base + (uint32_t(q * 32) << 16) + as * BN + c * 64;
-                uint32_t r[64];
-                {
-                    uint32_t (&r0)[32] = *reinterpret_cast<uint32_t(*)[32]>(&r[0]);
-                    uint32_t (&r1)[32] = *reinterpret_cast<uint32_t(*)[32]>(&r[32]);
-                    tmem_ld_x32(taddr, r0);
-                    tmem_ld_x32(taddr + 32, r1);
-                }
-                tmem_ld_wait();
-                if (c == NCHUNK - 1) { tc_fence_before(); mbar_arrive(&tmem_empty[as]); }
-                const int ncol0 = n0 + c * 64;
-                float v[64];
+            size_t out_row[2];
 #pragma unroll
-                for (int j = 0; j < 64; ++j) {
-                    float x = __uint_as_float(r[j]);
-                    if (p.bias != nullptr) x += __bfloat162float(p.bias[ncol0 + j]);
-                    v[j] = p.relu ? fmaxf(x, 0.f) : x;
+            for (int h = 0; h < 2; ++h) {
+                const int r = r_in + 8 * h;
+                if (MODE == 1) {
+                    out_row[h] = (size_t)mt * BM + r;
+                } else {   // tile row r = x + W * j, j = (image - b0) * TH + (row - y0) on the input grid
+                    const int j = r / p.W, x = r % p.W;
+                    out_row[h] = ((size_t)2 * (b0 * p.H + y0 + j) + p.py) * (2 * p.W) + 2 * x + p.px;
                 }
-                uint8_t* buf = epi_buf + (buf_sel & 1) * EPI_BYTES;
-                if (epi_tid == 0) tma_store_wait_read<1>();
-                named_bar_sync(1, 128);
-                uint8_t* rowp = buf + row * 128;
+            }
 #pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    uint4 o;
-                    o.x = pack_bf16x2(v[8 * j + 0], v[8 * j + 1]);
-                    o.y = pack_bf16x2(v[8 * j + 2], v[8 * j + 3]);
-                    o.z = pack_bf16x2(v[8 * j + 4], v[8 * j + 5]);
-                    o.w = pack_bf16x2(v[8 * j + 6], v[8 * j + 7]);
-                    *reinterpret_cast<uint4*>(rowp + ((j ^ (row & 7)) << 4)) = o;
+            for (int i = 0; i < BN / 8; ++i) {
+                const int col = n0 + 8 * i + c_in;
+                float b0f = 0.f, b1f = 0.f;
+                if (p.bias != nullptr) { b0f = __bfloat162float(p.bias[col]); b1f = __bfloat162float(p.bias[col + 1]); }
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    float v0 = acc[4 * i + 2 * h] + b0f, v1 = acc[4 * i + 2 * h + 1] + b1f;
+                    if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+                    *reinterpret_cast<uint32_t*>(p.y + out_row[h] * p.Cout + col) = pack_bf16x2(v0, v1);
                 }
-                fence_proxy_async_smem();
-                named_bar_sync(2, 128);
-                if (epi_tid == 0) {
-                    if (MODE == 1) tma_store_2d(&tmC, buf, ncol0, mt * BM);
-                    else tma_store_5d(&tmC, buf, ncol0, p.px, 0, p.py, b0 * p.H + y0);
-                    tma_store_commit();
-                }
-                ++buf_sel;
             }
         }
-        if (epi_tid == 0) tma_store_wait_all<0>();
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp_idx == 1) {
-        tc_fence_after();
-        tmem_dealloc<2 * BN>(tmem_base);
     }
 }
 
 bool pow2(int x) { return x > 0 && (x & (x - 1)) == 0; }
 
 template <int BN, int MODE>
-int launch_conv(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const ConvParams& p,
-                cudaStream_t s) {
+int launch_conv(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams& p, cudaStream_t s) {
     auto kern = conv_kernel<BN, MODE>;
     static bool attr_set = false;
     if (!attr_set) {
@@ -222,7 +186,7 @@ int launch_conv(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMa
     }
     const int tiles = p.num_m_tiles * p.num_n_blocks;
     const int grid = tiles < cvh::num_sms() ? tiles : cvh::num_sms();
-    kern<<<grid, NUM_THREADS, Cfg<BN>::SMEM_BYTES, s>>>(tmA, tmB, tmC, p);
+    kern<<<grid, NUM_THREADS, Cfg<BN>::SMEM_BYTES, s>>>(tmA, tmB, p);
     CV_LAUNCH_CHECK();
     return 0;
 }
@@ -256,7 +220,8 @@ extern "C" int cv_conv2d_k4s2(const void* x, const void* w_packed, const void* b
     p.relu = relu;
     const int BN = (Cout % 256 == 0) ? 256 : 128;
     p.num_n_blocks = Cout / BN;
-    alignas(64) CUtensorMap tmA, tmB, tmC;
+    p.y = static_cast<__nv_bfloat16*>(y);
+    alignas(64) CUtensorMap tmA, tmB;
     {   // input NHWC as [C, W, H, B], traversal stride 2 in W and H
         uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)IW, (uint64_t)IH, (uint64_t)B};
         uint64_t str[3] = {(uint64_t)Cin * 2, (uint64_t)IW * Cin * 2, (uint64_t)IH * IW * Cin * 2};
@@ -267,10 +232,8 @@ extern "C" int cv_conv2d_k4s2(const void* x, const void* w_packed, const void* b
     }
     int rc = cvh::encode_tmap_2d_bf16(&tmB, w_packed, (uint64_t)16 * Cout, Cin, Cin, BN, 64);
     if (rc) return rc;
-    rc = cvh::encode_tmap_2d_bf16(&tmC, y, (uint64_t)B * OH * OW, Cout, Cout, BM, 64);
-    if (rc) return rc;
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    return BN == 256 ? launch_conv<256, 1>(tmA, tmB, tmC, p, s) : launch_conv<128, 1>(tmA, tmB, tmC, p, s);
+    return BN == 256 ? launch_conv<256, 1>(tmA, tmB, p, s) : launch_conv<128, 1>(tmA, tmB, p, s);
 }
 
 extern "C" int cv_conv_transpose2d_k4s2(const void* x, const void* w_packed, const void* bias, void* y, int B, int IH,
@@ -283,7 +246,8 @@ extern "C" int cv_conv_transpose2d_k4s2(const void* x, const void* w_packed, con
     p.relu = relu;
     const int BN = (Cout % 256 == 0) ? 256 : 128;
     p.num_n_blocks = Cout / BN;
-    alignas(64) CUtensorMap tmA, tmB, tmC;
+    p.y = static_cast<__nv_bfloat16*>(y);
+    alignas(64) CUtensorMap tmA, tmB;
     {   // input NHWC as [C, W, H, B], unit strides; halo taps fall outside and are zero-filled
         uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)IW, (uint64_t)IH, (uint64_t)B};
         uint64_t str[3] = {(uint64_t)Cin * 2, (uint64_t)IW * Cin * 2, (uint64_t)IH * IW * Cin * 2};
@@ -294,18 +258,10 @@ extern "C" int cv_conv_transpose2d_k4s2(const void* x, const void* w_packed, con
     }
     int rc = cvh::encode_tmap_2d_bf16(&tmB, w_packed, (uint64_t)16 * Cout, Cin, Cin, BN, 64);
     if (rc) return rc;
-    {   // output [B, 2IH, 2IW, Cout] viewed as [C, px, b, py, (B*IH)]
-        const uint64_t OW = 2 * (uint64_t)IW;
-        uint64_t dims[5] = {(uint64_t)Cout, 2, (uint64_t)IW, 2, (uint64_t)B * IH};
-        uint64_t str[4] = {(uint64_t)Cout * 2, (uint64_t)2 * Cout * 2, OW * Cout * 2, 2 * OW * Cout * 2};
-        uint32_t box[5] = {64, 1, (uint32_t)IW, 1, (uint32_t)(p.TH * p.NB)};
-        rc = cvh::encode_tmap(&tmC, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, y, dims, str, box, nullptr, cvh::Swizzle::B128);
-        if (rc) return rc;
-    }
     cudaStream_t s = static_cast<cudaStream_t>(stream);
     for (int ph = 0; ph < 4; ++ph) {
         p.py = ph >> 1; p.px = ph & 1;
-        rc = BN == 256 ? launch_conv<256, 2>(tmA, tmB, tmC, p, s) : launch_conv<128, 2>(tmA, tmB, tmC, p, s);
+        rc = BN == 256 ? launch_conv<256, 2>(tmA, tmB, p, s) : launch_conv<128, 2>(tmA, tmB, p, s);
         if (rc) return rc;
     }
     return 0;

@@ -18,8 +18,8 @@ using namespace cv;
 // ------------------------------------------------------------------------------------------------
 // skinny linear on warp-level tensor-core MMAs (mma.sync m16n8k16, bf16 x bf16 -> fp32).
 //
-// 2 x 148 CTAs each own a contiguous, byte-balanced range of output columns (rows of W) walked in MMA tiles of 16;
-// the CTA's 8 warps split K, so even a 2560-column layer keeps 296 x 8 warps streaming.  Per 32-element K chunk a lane issues two 16-byte loads of W (rows g and g+8,
+// 2 CTAs per SM each own a contiguous, byte-balanced range of output columns (rows of W) walked in MMA tiles of 16;
+// the CTA's 8 warps split K, so even a 2560-column layer keeps 16 warps per SM streaming.  Per 32-element K chunk a lane issues two 16-byte loads of W (rows g and g+8,
 // elements 8q..8q+7; g = lane/4, q = lane%4) and one 16-byte load of x (row g): because a dot product does not
 // care in which order k is summed, those 8 contiguous elements are fed to two MMAs as the fragment slots
 // {2q,2q+1,2q+8,2q+9}, with x permuted identically — so both operands are read with full 16-byte, sector-exact
@@ -60,8 +60,8 @@ __device__ __forceinline__ void mma_bf16_16816(float (&d)[4], uint32_t a0, uint3
 }
 
 // WIDE: 9..16 rows of x — a second B fragment set (rows 8..15) and a second accumulator reuse the same weight
-// fragments, so the weights are still streamed ONCE (two passes of the 8-row kernel doubled the decode step time at
-// batch 16: 7.8 ms vs 3.8 ms at batch 8); half the K chunks in flight per warp keeps the register count.
+// fragments, so the weights are still streamed ONCE (two passes of the 8-row kernel would stream them twice); half the
+// K chunks in flight per warp keeps the register count.
 template <int UNROLL, bool WIDE>
 struct SkStage {
     uint4 w0[UNROLL], w1[UNROLL], xv[UNROLL], xw[WIDE ? UNROLL : 1];
@@ -576,9 +576,8 @@ extern "C" int cv_linear_small_m(const void* x, int64_t ldx, const void* W, int6
         cvh::count_launches(1);
         return 0;
     }
-    // COGVIEW_B200_LINEAR_RING=1: the bulk-copy-ring kernel (csrc/linear_ring.cu) for M <= 8.  Parity-green, but in
-    // the 4B decode step it measured 3.10 ms per token against 2.91 ms for the fragment-direct kernel below (the step
-    // is bound by the latency of its ~340 dependent launches, not by the streaming rate of one of them): opt-in.
+    // COGVIEW_B200_LINEAR_RING=1: the bulk-copy-ring kernel (csrc/linear_ring.cu) for M <= 8.  Parity-green, opt-in:
+    // the decode step is bound by the latency of its ~340 dependent launches, not by the streaming rate of one of them.
     static int use_ring = -1;
     if (use_ring < 0) {
         const char* e = getenv("COGVIEW_B200_LINEAR_RING");
@@ -690,7 +689,7 @@ extern "C" int cv_attn_gather(const void* q, int64_t ldq, int64_t bsq, const voi
 // Sparse inference on the device (is_sparse == 2, mpu/sparse_transformer.py:498-520, :591-600): the index plan of one
 // decode step for EVERY layer in one launch.  Per (layer, sequence): all text positions before the trailing window plus a
 // uniformly random subset of the image positions before it (num_pivot entries in total), then the window.  The reference
-// draws the subset with Python's random.sample per layer per token on the host (50 ms per token at 3000 positions);
+// draws the subset with Python's random.sample per layer per token on the host;
 // here every candidate gets a counter-based random key and the smallest keys win — the same distribution (a uniformly
 // random k-subset, fresh per layer and token), a different random stream.  One 64-bit bitonic sort per CTA orders
 // "text first (key 0), then images by random key"; the first num_pivot entries are the pivots.

@@ -6,7 +6,7 @@
 // y + LN4 (mpu/sparse_transformer.py:314-342), then the final LayerNorm and the tied-embedding logits.
 //
 // The step is HBM bound: 7.86 GB of bf16 weights are read once per step (SURVEY §8(d)).  Launching one small kernel
-// per linear leaves every launch in its ramp-up / drain (14 us for a 6 us-ideal launch, profiles/r01_*linear*), so:
+// per linear leaves every launch in its ramp-up / drain, so:
 //
 //   * one CTA per SM, resident for the whole step: 16 consumer warps + 1 producer warp;
 //   * every weight matrix is split into contiguous row ranges, one per CTA;
@@ -27,8 +27,7 @@
 //   * the fp32 residual stream never leaves the SM: every CTA keeps the full [M, h] stream in REGISTERS (20 floats per
 //     thread at M <= 4) and computes the Sandwich-LN glue (two abs-max LayerNorms + residual,
 //     mpu/sparse_transformer.py:40-44) redundantly straight into its shared-memory operand.  The only thing a glue reads
-//     from other SMs is the bf16 output of the preceding linear (20 KB at M = 4): a version that kept the stream in L2
-//     moved 123 KB per CTA per glue = 18 MB through L2 at once and took 7 us per glue, most of it L2 bandwidth;
+//     from other SMs is the bf16 output of the preceding linear (20 KB at M = 4), not the whole residual stream;
 //   * attention over the K|V cache runs on (sequence, head, key-block) units, balanced over the CTAs as one flattened
 //     range; a (sequence, head) pair that straddles CTAs is merged by the CTA that owns its FIRST key blocks — which
 //     it processes LAST, so the other contributors' partial states (plain stores + one release-add) are already there:
@@ -380,8 +379,8 @@ __global__ void __launch_bounds__(NT, 1) decode_step_kernel(const __grid_constan
 
     // ============================================================================================
     // epilogue warp: sums the 16 K-slice partials of every finished [16 outputs x 8 sequences] tile, applies bias /
-    // GELU and stores — off the consumers' critical path (a CTA-wide bar.sync + reduce per tile cost the consumers
-    // 0.46 us per 82 KB tile: tools/micro/consume_bench.cu).  part[pbuf] is handed over with named barriers:
+    // GELU and stores — off the consumers' critical path (a CTA-wide bar.sync + reduce per tile would stall every
+    // consumer warp).  part[pbuf] is handed over with named barriers:
     // consumers bar.arrive PFULL after writing, this warp bar.arrive PFREE after reading.
     // ============================================================================================
     if (warp == CW + 1) {

@@ -7,11 +7,11 @@
 //   logits GEMM                   /root/reference/model/gpt2_modeling.py:117-118
 // and their autograd backward (dgrad: B MN-major; wgrad: A and B MN-major).
 //
-// Design (sm_100a): persistent, one CTA per SM, 6 warps.
-//   warp 0      TMA producer: cp.async.bulk.tensor tiles -> 128B-swizzled smem ring (4-6 stages)
-//   warp 1      MMA issuer: one elected thread issues tcgen05.mma (M=128, N=BN, K=16) into TMEM;
-//               two accumulator stages (2 x BN columns) so the epilogue of tile i overlaps tile i+1
-//   warps 2-5   epilogue: tcgen05.ld -> bias/GELU/abs-max -> each thread stores its row's 128 B straight to global
+// Design (sm_90a): persistent, one CTA per SM, 3 warpgroups.
+//   warpgroup 0     TMA producer (one thread): cp.async.bulk.tensor tiles -> 128B-swizzled smem ring (4-6 stages)
+//   warpgroups 1-2  wgmma consumers: each owns 64 rows of the 128-row tile (m64 x BN x k16, fp32 accumulators in
+//                   registers), then applies bias / activation / dropout / abs-max and stores its rows straight to
+//                   global memory while the producer already streams the next tile's operands into the ring
 #include <cstdlib>
 
 #include "common.cuh"
@@ -24,7 +24,7 @@ using namespace cv;
 
 constexpr int BM = 128;
 constexpr int BK = 64;
-constexpr int NUM_THREADS = 192;
+constexpr int NUM_THREADS = 384;
 
 template <int BN>
 struct Cfg {
@@ -32,8 +32,7 @@ struct Cfg {
     static constexpr int B_BYTES = BN * BK * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
     static constexpr int STAGES = (BN == 256) ? 4 : 6;
-    static constexpr int CSTAGE_BYTES = 4 * 2 * 4096;   // C staging: 4 epilogue warps x 2 buffers x [32 rows x 128 B]
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + CSTAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 };
 
 struct GemmParams {
@@ -50,14 +49,11 @@ struct GemmParams {
     void* c;                    // output [M, N] (bf16 or fp32), leading dimension ldc
     __nv_bfloat16* c2;          // optional pre-activation output (bf16, same ldc)
     int64_t ldc;
-    int vec32;                  // C and C2 rows start 32-byte aligned: 256-bit stores
-    int tma_store;              // C (and C2) go through shared memory + cp.async.bulk.tensor stores (whole 128-byte lines)
-    int dbg;                    // timing experiments (COGVIEW_B200_GEMM_DBG): 1 = no global stores, 2 = no TMEM loads
 };
 
 // Tail-wave splitting: with T tiles on G persistent CTAs the last T % G tiles would occupy a whole wave while most
-// SMs idle (34 x 10 = 340 tiles of a 4352 x 2560 output on 148 SMs: 2.3 waves cost 3).  When those r tiles fit twice
-// (2r <= G) they are issued as 2r half-width tiles instead, so the last wave costs one half tile (~0.75 of a full one).
+// SMs idle (34 x 10 = 340 tiles of a 4352 x 2560 output on 132 SMs: 2.6 waves cost 3).  When those r tiles fit twice
+// (2r <= G) they are issued as 2r half-width tiles instead, so the last wave costs one half tile.
 struct TileCoord { int m0, n0, width; };
 template <int BN>
 __device__ __forceinline__ TileCoord tile_coord(const GemmParams& p, int tile) {
@@ -76,88 +72,67 @@ __device__ __forceinline__ TileCoord tile_coord(const GemmParams& p, int tile) {
     return t;
 }
 
-// 32-byte (whole-sector) global store: the epilogue threads write rows that are kilobytes apart, so a 16-byte store is
-// half a sector per lane — with 16-byte stores the C writes cost 14 % of the QKV GEMM (128 us; 110 us with the stores
-// compiled out, tools/gemm_dbg_bench.py)
-__device__ __forceinline__ uint32_t r_as_u32(float x) { return __float_as_uint(x); }
-__device__ __forceinline__ void st_global_v8(void* p, uint32_t a, uint32_t b, uint32_t c, uint32_t d, uint32_t e, uint32_t f,
-                                             uint32_t g, uint32_t h) {
-    asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(a), "r"(b), "r"(c), "r"(d), "r"(e),
-                 "r"(f), "r"(g), "r"(h) : "memory");
+// dropout4 for the two consecutive elements idx, idx + 1 (idx even) that one accumulator fragment holds: the same
+// Philox call (counter idx / 4), words x, y or z, w
+__device__ __forceinline__ void dropout2(const DropoutArgs& d, uint64_t idx, float& a, float& b) {
+    const uint4 r = philox4x32_10(d.seed, idx >> 2, d.stream);
+    const uint32_t ra = (idx & 2) ? r.z : r.x, rb = (idx & 2) ? r.w : r.y;
+    a = ra >= d.threshold ? a * d.scale : 0.f;
+    b = rb >= d.threshold ? b * d.scale : 0.f;
 }
-// 16 consecutive bf16 outputs of one row: one 32-byte store when the row is 32-byte aligned and the group is inside
-// [0, N), else two 16-byte groups / scalar tail
-__device__ __forceinline__ void store_bf16x16(__nv_bfloat16* dst, const float* v, int n, int N, bool vec32, bool n_vec_ok) {
-    if (vec32 && n + 16 <= N) {
-        st_global_v8(dst, pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]),
-                     pack_bf16x2(v[8], v[9]), pack_bf16x2(v[10], v[11]), pack_bf16x2(v[12], v[13]), pack_bf16x2(v[14], v[15]));
-        return;
-    }
-#pragma unroll
-    for (int hgrp = 0; hgrp < 2; ++hgrp) {
-        const int nn = n + hgrp * 8;
-        const float* vv = v + hgrp * 8;
-        if (n_vec_ok && nn + 8 <= N) {
-            uint4 o;
-            o.x = pack_bf16x2(vv[0], vv[1]); o.y = pack_bf16x2(vv[2], vv[3]);
-            o.z = pack_bf16x2(vv[4], vv[5]); o.w = pack_bf16x2(vv[6], vv[7]);
-            *reinterpret_cast<uint4*>(dst + hgrp * 8) = o;
-        } else {
-#pragma unroll
-            for (int t = 0; t < 8; ++t)
-                if (nn + t < N) dst[hgrp * 8 + t] = __float2bfloat16_rn(vv[t]);
-        }
-    }
+
+template <int N, int TA, int TB>
+__device__ __forceinline__ void mma_n(float* acc, uint64_t da, uint64_t db, uint32_t sc) {
+    if constexpr (N == 256) wgmma_ss_n256<TA, TB>(*reinterpret_cast<float(*)[128]>(acc), da, db, sc);
+    else if constexpr (N == 128) wgmma_ss_n128<TA, TB>(*reinterpret_cast<float(*)[64]>(acc), da, db, sc);
+    else wgmma_ss_n64<TA, TB>(*reinterpret_cast<float(*)[32]>(acc), da, db, sc);
+}
+
+__device__ __forceinline__ void store_pair(__nv_bfloat16* dst, float a, float b, bool pair) {
+    if (pair) *reinterpret_cast<uint32_t*>(dst) = pack_bf16x2(a, b);
+    else dst[0] = __float2bfloat16_rn(a);
+}
+__device__ __forceinline__ void store_pair(float* dst, float a, float b, bool pair) {
+    if (pair) *reinterpret_cast<float2*>(dst) = make_float2(a, b);
+    else dst[0] = a;
 }
 
 template <int BN, bool A_MN, bool B_MN, bool OUT_F32>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-            const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmC2, const GemmParams p) {
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
     using C = Cfg<BN>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* smem_c = smem + C::STAGES * C::STAGE_BYTES;     // 1024-byte aligned (stage sizes are multiples of 1024)
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem_c + C::CSTAGE_BYTES);
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);
     uint64_t* full_bar = bars;                       // [STAGES]
-    uint64_t* empty_bar = bars + C::STAGES;          // [STAGES]
-    uint64_t* tmem_full = bars + 2 * C::STAGES;      // [2]
-    uint64_t* tmem_empty = bars + 2 * C::STAGES + 2; // [2]
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * C::STAGES + 4);
+    uint64_t* empty_bar = bars + C::STAGES;          // [STAGES]: one arrive per consumer warp
 
-    const int warp_idx = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7;
+    const int tid = threadIdx.x & 127;
     const int num_tiles = p.num_tiles;
 
-    if (warp_idx == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmB);
         for (int i = 0; i < C::STAGES; ++i) {
             mbar_init(&full_bar[i], 1);
-            mbar_init(&empty_bar[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&tmem_full[i], 1);
-            mbar_init(&tmem_empty[i], 128);
+            mbar_init(&empty_bar[i], 8);
         }
         fence_barrier_init();
     }
-    if (warp_idx == 1) tmem_alloc<2 * BN>(tmem_ptr);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
 
-    if (warp_idx == 0) {
+    if (wg == 0) {
         // ------------------------------ TMA producer ------------------------------
-        if (lane == 0) {
+        setmaxnreg_dec<40>();
+        if (tid == 0) {
             int stage = 0;
             uint32_t phase = 0;
             for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
                 const TileCoord tc = tile_coord<BN>(p, tile);
                 const int m0 = tc.m0, n0 = tc.n0;
                 for (int kb = 0; kb < p.num_k_blocks; ++kb) {
-                    mbar_wait(&empty_bar[stage], phase ^ 1);
+                    mbar_wait<false>(&empty_bar[stage], phase ^ 1);
                     uint8_t* sA = smem + stage * C::STAGE_BYTES;
                     uint8_t* sB = sA + C::A_BYTES;
                     mbar_expect_tx(&full_bar[stage], C::A_BYTES + tc.width * BK * 2);
@@ -183,226 +158,88 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                 }
             }
         }
-    } else if (warp_idx == 1) {
-        // ------------------------------ MMA issuer ------------------------------
-        if (lane == 0) {
-            constexpr uint32_t idesc_full = make_idesc_bf16(BM, BN, A_MN ? 1u : 0u, B_MN ? 1u : 0u);
-            constexpr uint32_t idesc_half = make_idesc_bf16(BM, BN / 2, A_MN ? 1u : 0u, B_MN ? 1u : 0u);
-            // K-major: 8-row groups 1024 B apart. MN-major: 64-element chunks one TMA box (BK*128 B) apart,
-            // 8-row K groups 1024 B apart.
-            constexpr uint32_t A_LBO = A_MN ? BK * 128 : 0, B_LBO = B_MN ? BK * 128 : 0;
-            constexpr uint32_t A_KSTEP = A_MN ? 16 * 128 : 32, B_KSTEP = B_MN ? 16 * 128 : 32;
-            int stage = 0;
-            uint32_t phase = 0;
-            int it = 0;
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-                const int as = it & 1;
-                const uint32_t aphase = (it >> 1) & 1;
-                const uint32_t idesc = tile < p.split_from ? idesc_full : idesc_half;
-                mbar_wait(&tmem_empty[as], aphase ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + as * BN;
-                for (int kb = 0; kb < p.num_k_blocks; ++kb) {
-                    mbar_wait(&full_bar[stage], phase);
-                    tc_fence_after();
-                    const uint32_t a_addr = smem_u32(smem + stage * C::STAGE_BYTES);
-                    const uint32_t b_addr = a_addr + C::A_BYTES;
-#pragma unroll
-                    for (int k = 0; k < BK / 16; ++k) {
-                        const uint64_t da = make_smem_desc_sw128(a_addr + k * A_KSTEP, A_LBO, 1024);
-                        const uint64_t db = make_smem_desc_sw128(b_addr + k * B_KSTEP, B_LBO, 1024);
-                        umma_f16(d_tmem, da, db, idesc, (kb | k) != 0 ? 1u : 0u);
-                    }
-                    umma_commit(&empty_bar[stage]);  // smem slot reusable once these MMAs retire
-                    if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-                }
-                umma_commit(&tmem_full[as]);  // accumulator complete
-            }
-        }
     } else {
-        // ------------------------------ epilogue warps ------------------------------
-        // Each thread owns one accumulator row: it reads 64 (bf16 out) or 32 (fp32 out) columns from TMEM, applies
-        // bias / activation / abs-max and writes its 128 contiguous bytes of C straight to global memory (whole
-        // cache lines per thread) — no staging buffer, no barriers: the four warps run fully decoupled, so the
-        // epilogue of tile i stays hidden under the MMAs of tile i+1.
-        const int q = warp_idx & 3;             // TMEM lane quadrant this warp may access
-        const int row = q * 32 + lane;          // row within the tile
-        constexpr int EPI_COLS = OUT_F32 ? 32 : 64;
-        const bool n_vec_ok = (p.N % 8) == 0;   // whole 16-byte groups are either inside or outside [0, N)
-        // TMA-store path: the lane's 128-byte row of a chunk goes to this warp's 128B-swizzled [32 x 128 B] staging buffer
-        // (double-buffered), lane 0 issues one cp.async.bulk.tensor store per chunk: whole 128-byte lines leave the SM
-        // asynchronously instead of 32 scattered sector writes per store instruction; rows / columns outside C are
-        // clipped by the tensor map.
-        uint8_t* sC = smem_c + q * 8192;
-        int cc = 0;
-        auto put_row = [&](const CUtensorMap* tm, const float* vals, int col0, int row0) {
-            uint8_t* buf = sC + (cc & 1) * 4096;
-            if (cc >= 2) {
-                if (lane == 0) tma_store_wait_read<1>();
-                __syncwarp();
-            }
-            uint8_t* rowp = buf + lane * 128;
+        // ------------------------------ wgmma consumers + epilogue ------------------------------
+        setmaxnreg_inc<232>();
+        const int half = wg - 1;                            // rows 64 half .. 64 half + 63 of the tile
+        const int warp = tid >> 5, lane = tid & 31;
+        const int r_in = 64 * half + 16 * warp + (lane >> 2);   // this thread's rows: r_in and r_in + 8
+        const int c_in = 2 * (lane & 3);                    // and columns 8i + c_in, + 1
+        // K-major: 8-row groups 1024 B apart. MN-major: 64-element chunks one TMA box (BK*128 B) apart,
+        // 8-row K groups 1024 B apart.
+        constexpr uint32_t A_LBO = A_MN ? BK * 128 : 0, B_LBO = B_MN ? BK * 128 : 0;
+        constexpr uint32_t A_KSTEP = A_MN ? 16 * 128 : 32, B_KSTEP = B_MN ? 16 * 128 : 32;
+        const uint32_t a_half = A_MN ? half * (BK * 128) : half * (64 * 128);
+        constexpr int TA = A_MN ? 1 : 0, TB = B_MN ? 1 : 0;
+        int stage = 0;
+        uint32_t phase = 0;
+        float acc[BN / 2];
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                uint4 o;
-                if (OUT_F32) {
-                    o.x = __float_as_uint(vals[4 * j]); o.y = __float_as_uint(vals[4 * j + 1]);
-                    o.z = __float_as_uint(vals[4 * j + 2]); o.w = __float_as_uint(vals[4 * j + 3]);
-                } else {
-                    o.x = pack_bf16x2(vals[8 * j + 0], vals[8 * j + 1]); o.y = pack_bf16x2(vals[8 * j + 2], vals[8 * j + 3]);
-                    o.z = pack_bf16x2(vals[8 * j + 4], vals[8 * j + 5]); o.w = pack_bf16x2(vals[8 * j + 6], vals[8 * j + 7]);
-                }
-                *reinterpret_cast<uint4*>(rowp + ((j ^ (lane & 7)) << 4)) = o;
-            }
-            fence_proxy_async_smem();
-            __syncwarp();
-            if (lane == 0) {
-                tma_store_2d(tm, buf, col0, row0);
-                tma_store_commit();
-            }
-            ++cc;
-        };
-        int it = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
             const TileCoord tc = tile_coord<BN>(p, tile);
+            const bool full = tc.width == BN;
+            int prev = -1;
+            for (int kb = 0; kb < p.num_k_blocks; ++kb) {
+                mbar_wait<false>(&full_bar[stage], phase);
+                const uint32_t a_addr = smem_u32(smem + stage * C::STAGE_BYTES) + a_half;
+                const uint32_t b_addr = smem_u32(smem + stage * C::STAGE_BYTES + C::A_BYTES);
+                fence_regs(acc);
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BK / 16; ++k) {
+                    const uint64_t da = make_smem_desc_sw128(a_addr + k * A_KSTEP, A_LBO, 1024);
+                    const uint64_t db = make_smem_desc_sw128(b_addr + k * B_KSTEP, B_LBO, 1024);
+                    const uint32_t sc = (kb | k) != 0 ? 1u : 0u;
+                    if (full) mma_n<BN, TA, TB>(acc, da, db, sc);
+                    else mma_n<BN / 2, TA, TB>(acc, da, db, sc);
+                }
+                wgmma_commit();
+                wgmma_wait<1>();                            // the previous k-block's MMAs retired: free its slot
+                if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+                prev = stage;
+                if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
+            }
+            wgmma_wait<0>();
+            fence_regs(acc);
+            if (lane == 0) mbar_arrive(&empty_bar[prev]);
+
             const int m0 = tc.m0, n0 = tc.n0;
-            const int nchunk = tc.width / EPI_COLS;
-            const int as = it & 1;
-            const uint32_t aphase = (it >> 1) & 1;
-            mbar_wait(&tmem_full[as], aphase);
-            tc_fence_after();
-            const int grow = m0 + row;
-            const bool row_ok = grow < p.M;
             float tmax = 0.f;
-#pragma unroll 1
-            for (int c = 0; c < nchunk; ++c) {
-                const uint32_t taddr = tmem_base + (uint32_t(q * 32) << 16) + as * BN + c * EPI_COLS;
-                uint32_t r[EPI_COLS];
-                if (p.dbg & 2) {
 #pragma unroll
-                    for (int j = 0; j < EPI_COLS; ++j) r[j] = j + c;
-                } else {
-                    uint32_t (&r0)[32] = *reinterpret_cast<uint32_t(*)[32]>(&r[0]);
-                    tmem_ld_x32(taddr, r0);
-                    if (EPI_COLS == 64) {
-                        uint32_t (&r1)[32] = *reinterpret_cast<uint32_t(*)[32]>(&r[EPI_COLS - 32]);
-                        tmem_ld_x32(taddr + 32, r1);
-                    }
-                }
-                tmem_ld_wait();
-                if (c == nchunk - 1) {
-                    // all TMEM reads of this accumulator stage are done -> hand it back to the MMA warp
-                    tc_fence_before();
-                    mbar_arrive(&tmem_empty[as]);
-                }
-                const int ncol0 = n0 + c * EPI_COLS;
-                float v[EPI_COLS];
-#pragma unroll
-                for (int j = 0; j < EPI_COLS; ++j) v[j] = __uint_as_float(r[j]);
+            for (int i = 0; i < BN / 8; ++i) {
+                if (i * 8 >= tc.width) break;
+                const int col = n0 + 8 * i + c_in;
+                if (col >= p.N) continue;
+                const bool pair = col + 1 < p.N;
+                float b0 = 0.f, b1 = 0.f;
                 if (p.bias != nullptr) {
-#pragma unroll
-                    for (int g = 0; g < EPI_COLS / 8; ++g) {
-                        const int n = ncol0 + g * 8;
-                        if (n_vec_ok && n + 8 <= p.N) {       // one broadcast 16-byte load per 8 columns
-                            const uint4 u = __ldg(reinterpret_cast<const uint4*>(p.bias + n));
-                            const __nv_bfloat162* b2 = reinterpret_cast<const __nv_bfloat162*>(&u);
-#pragma unroll
-                            for (int t = 0; t < 4; ++t) {
-                                v[g * 8 + 2 * t] += __low2float(b2[t]);
-                                v[g * 8 + 2 * t + 1] += __high2float(b2[t]);
-                            }
-                        } else {
-#pragma unroll
-                            for (int t = 0; t < 8; ++t)
-                                if (n + t < p.N) v[g * 8 + t] += __bfloat162float(p.bias[n + t]);
-                        }
-                    }
+                    b0 = __bfloat162float(p.bias[col]);
+                    if (pair) b1 = __bfloat162float(p.bias[col + 1]);
                 }
-                if (p.has_c2 && p.tma_store) {
-                    put_row(&tmC2, v, ncol0, m0 + q * 32);
-                } else if (p.has_c2 && row_ok) {   // pre-activation copy (bf16)
-                    __nv_bfloat16* dst = p.c2 + (size_t)grow * p.ldc + ncol0;
 #pragma unroll
-                    for (int g = 0; g < EPI_COLS / 16; ++g)
-                        store_bf16x16(dst + g * 16, v + g * 16, ncol0 + g * 16, p.N, p.vec32 != 0, n_vec_ok);
-                }
-                if (p.act == 1) {
-#pragma unroll
-                    for (int j = 0; j < EPI_COLS; ++j) v[j] = gelu_tanh_fast(v[j]);
-                } else if (p.act == 2) {
-#pragma unroll
-                    for (int j = 0; j < EPI_COLS; ++j) v[j] = fmaxf(v[j], 0.f);
-                } else if (p.act == 3 && row_ok) {
-                    const __nv_bfloat16* ax = p.aux + (size_t)grow * p.ldc + ncol0;
-#pragma unroll
-                    for (int g = 0; g < EPI_COLS / 8; ++g) {
-                        const int n = ncol0 + g * 8;
-                        if (n_vec_ok && n + 8 <= p.N) {
-                            const uint4 u = *reinterpret_cast<const uint4*>(ax + g * 8);
-                            const __nv_bfloat162* a2 = reinterpret_cast<const __nv_bfloat162*>(&u);
-#pragma unroll
-                            for (int t = 0; t < 4; ++t) {
-                                v[g * 8 + 2 * t] *= gelu_tanh_grad(__low2float(a2[t]));
-                                v[g * 8 + 2 * t + 1] *= gelu_tanh_grad(__high2float(a2[t]));
-                            }
-                        } else {
-#pragma unroll
-                            for (int t = 0; t < 8; ++t)
-                                if (n + t < p.N) v[g * 8 + t] *= gelu_tanh_grad(__bfloat162float(ax[g * 8 + t]));
-                        }
+                for (int h = 0; h < 2; ++h) {
+                    const int row = m0 + r_in + 8 * h;
+                    if (row >= p.M) continue;
+                    float v0 = acc[4 * i + 2 * h] + b0, v1 = acc[4 * i + 2 * h + 1] + b1;
+                    const size_t off = (size_t)row * p.ldc + col;
+                    if (p.has_c2) store_pair(p.c2 + off, v0, v1, pair);     // pre-activation copy (bf16)
+                    if (p.act == 1) {
+                        v0 = gelu_tanh_fast(v0); v1 = gelu_tanh_fast(v1);
+                    } else if (p.act == 2) {
+                        v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f);
+                    } else if (p.act == 3) {
+                        v0 *= gelu_tanh_grad(__bfloat162float(p.aux[off]));
+                        if (pair) v1 *= gelu_tanh_grad(__bfloat162float(p.aux[off + 1]));
                     }
-                }
-                if (p.drop.p > 0.f) {
-#pragma unroll
-                    for (int g4 = 0; g4 < EPI_COLS / 4; ++g4) {
-                        const uint64_t idx4 = ((uint64_t)grow * p.N + ncol0 + g4 * 4) >> 2;
-                        dropout4(p.drop, idx4, v[4 * g4], v[4 * g4 + 1], v[4 * g4 + 2], v[4 * g4 + 3]);
-                    }
-                }
-                if (p.tma_store && !(p.dbg & 1)) {
-                    put_row(&tmC, v, ncol0, m0 + q * 32);
-                    if (p.absmax != nullptr && row_ok) {
-#pragma unroll
-                        for (int j = 0; j < EPI_COLS; ++j)
-                            if (ncol0 + j < p.N) tmax = fmaxf(tmax, fabsf(OUT_F32 ? v[j] : bf16_round(v[j])));
-                    }
-                } else if (row_ok && !(p.dbg & 1)) {
+                    if (p.drop.p > 0.f) dropout2(p.drop, (uint64_t)row * p.N + col, v0, v1);
                     if (OUT_F32) {
-                        float* dst = static_cast<float*>(p.c) + (size_t)grow * p.ldc + ncol0;
-#pragma unroll
-                        for (int g = 0; g < EPI_COLS / 4; ++g) {
-                            const int n = ncol0 + g * 4;
-                            if (p.vec32 && (g & 1) == 0 && n + 8 <= p.N) {
-                                st_global_v8(dst + g * 4, r_as_u32(v[4 * g]), r_as_u32(v[4 * g + 1]), r_as_u32(v[4 * g + 2]),
-                                             r_as_u32(v[4 * g + 3]), r_as_u32(v[4 * g + 4]), r_as_u32(v[4 * g + 5]),
-                                             r_as_u32(v[4 * g + 6]), r_as_u32(v[4 * g + 7]));
-                            } else if (p.vec32 && (g & 1) == 1 && n + 4 <= p.N) {
-                                // written with the previous group (n - 4 + 8 <= N)
-                            } else if ((p.N % 4) == 0 && n + 4 <= p.N) {
-                                *reinterpret_cast<float4*>(dst + g * 4) =
-                                    make_float4(v[4 * g], v[4 * g + 1], v[4 * g + 2], v[4 * g + 3]);
-                            } else {
-#pragma unroll
-                                for (int t = 0; t < 4; ++t)
-                                    if (n + t < p.N) dst[g * 4 + t] = v[4 * g + t];
-                            }
-                        }
-                        if (p.absmax != nullptr) {
-#pragma unroll
-                            for (int j = 0; j < EPI_COLS; ++j)
-                                if (ncol0 + j < p.N) tmax = fmaxf(tmax, fabsf(v[j]));
-                        }
+                        store_pair(static_cast<float*>(p.c) + off, v0, v1, pair);
                     } else {
-                        __nv_bfloat16* dst = static_cast<__nv_bfloat16*>(p.c) + (size_t)grow * p.ldc + ncol0;
-#pragma unroll
-                        for (int g = 0; g < EPI_COLS / 16; ++g)
-                            store_bf16x16(dst + g * 16, v + g * 16, ncol0 + g * 16, p.N, p.vec32 != 0, n_vec_ok);
-                        if (p.absmax != nullptr) {
-#pragma unroll
-                            for (int j = 0; j < EPI_COLS; ++j)
-                                if (ncol0 + j < p.N) tmax = fmaxf(tmax, fabsf(bf16_round(v[j])));
-                        }
+                        store_pair(static_cast<__nv_bfloat16*>(p.c) + off, v0, v1, pair);
+                        v0 = bf16_round(v0); v1 = bf16_round(v1);
                     }
+                    if (p.absmax != nullptr) tmax = fmaxf(tmax, fmaxf(fabsf(v0), pair ? fabsf(v1) : 0.f));
                 }
             }
             if (p.absmax != nullptr) {
@@ -410,20 +247,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                 if (lane == 0 && tmax > 0.f) atomic_max_nonneg(p.absmax, tmax);
             }
         }
-        if (p.tma_store && lane == 0) tma_store_wait_read<0>();   // the staging buffers must outlive their readers
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp_idx == 1) {
-        tc_fence_after();
-        tmem_dealloc<2 * BN>(tmem_base);
     }
 }
 
 template <int BN, bool A_MN, bool B_MN, bool OUT_F32>
-int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, const CUtensorMap& tmC2,
-           const GemmParams& p, cudaStream_t stream) {
+int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t stream) {
     auto kern = gemm_kernel<BN, A_MN, B_MN, OUT_F32>;
     static bool attr_set = false;
     if (!attr_set) {
@@ -433,7 +261,7 @@ int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tm
     }
     int tiles = p.num_tiles;
     int grid = tiles < cvh::gemm_sms() ? tiles : cvh::gemm_sms();
-    kern<<<grid, NUM_THREADS, Cfg<BN>::SMEM_BYTES, stream>>>(tmA, tmB, tmC, tmC2, p);
+    kern<<<grid, NUM_THREADS, Cfg<BN>::SMEM_BYTES, stream>>>(tmA, tmB, p);
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return cvh::fail_cuda("cv_gemm_bf16", e);
     cvh::count_launches(1);
@@ -441,17 +269,17 @@ int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tm
 }
 
 template <int BN>
-int dispatch(int a_mn, int b_mn, int out_f32, const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC,
-             const CUtensorMap& tmC2, const GemmParams& p, cudaStream_t s) {
+int dispatch(int a_mn, int b_mn, int out_f32, const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p,
+             cudaStream_t s) {
     if (out_f32) {
-        if (!a_mn && !b_mn) return launch<BN, false, false, true>(tmA, tmB, tmC, tmC2, p, s);
-        if (!a_mn && b_mn) return launch<BN, false, true, true>(tmA, tmB, tmC, tmC2, p, s);
-        if (a_mn && b_mn) return launch<BN, true, true, true>(tmA, tmB, tmC, tmC2, p, s);
+        if (!a_mn && !b_mn) return launch<BN, false, false, true>(tmA, tmB, p, s);
+        if (!a_mn && b_mn) return launch<BN, false, true, true>(tmA, tmB, p, s);
+        if (a_mn && b_mn) return launch<BN, true, true, true>(tmA, tmB, p, s);
         return cvh::fail_arg("cv_gemm_bf16", "A MN-major with B K-major is not instantiated");
     }
-    if (!a_mn && !b_mn) return launch<BN, false, false, false>(tmA, tmB, tmC, tmC2, p, s);
-    if (!a_mn && b_mn) return launch<BN, false, true, false>(tmA, tmB, tmC, tmC2, p, s);
-    if (a_mn && b_mn) return launch<BN, true, true, false>(tmA, tmB, tmC, tmC2, p, s);
+    if (!a_mn && !b_mn) return launch<BN, false, false, false>(tmA, tmB, p, s);
+    if (!a_mn && b_mn) return launch<BN, false, true, false>(tmA, tmB, p, s);
+    if (a_mn && b_mn) return launch<BN, true, true, false>(tmA, tmB, p, s);
     return cvh::fail_arg("cv_gemm_bf16", "A MN-major with B K-major is not instantiated");
 }
 
@@ -482,9 +310,8 @@ static int gemm_impl(const void* A, int a_mn_major, int64_t lda, const void* B, 
 
     int BN = block_n;
     if (BN == 0) {
-        // Estimated time = waves x per-tile cost.  A 128x128 tile needs as many shared-memory operand bytes per
-        // MMA cycle as the SM can deliver (128 B/clk), so it runs at ~2/3 of the 128x256 tile's per-column rate
-        // (measured: ~0.9 vs ~1.4 PFLOP/s): cost 192 vs 256 per tile.
+        // Estimated time = waves x per-tile cost.  A 128x128 tile streams as many operand bytes per output column as
+        // a 128x256 tile streams for two, so it is modelled at 3/4 of the wide tile's cost: 192 vs 256 per tile.
         // With tail-wave splitting (tile_coord) the last partial wave of the 256-wide schedule costs one 128-wide
         // tile when its tiles fit twice on the SMs.
         const int sms = cvh::gemm_sms();
@@ -521,13 +348,6 @@ static int gemm_impl(const void* A, int a_mn_major, int64_t lda, const void* B, 
     p.c = Cout;
     p.c2 = static_cast<__nv_bfloat16*>(C2);
     p.ldc = ldc;
-    {
-        static const int dbg = [] { const char* e = getenv("COGVIEW_B200_GEMM_DBG"); return e ? atoi(e) : 0; }();
-        p.dbg = dbg;
-        const size_t esz = c_is_f32 ? 4 : 2;
-        p.vec32 = !(dbg & 4) && (reinterpret_cast<uintptr_t>(Cout) % 32 == 0) && ((ldc * esz) % 32 == 0) &&
-                  (C2 == nullptr || (reinterpret_cast<uintptr_t>(C2) % 32 == 0 && (ldc * 2) % 32 == 0));
-    }
 
     alignas(64) CUtensorMap tmA, tmB;
     int rc;
@@ -538,23 +358,8 @@ static int gemm_impl(const void* A, int a_mn_major, int64_t lda, const void* B, 
     rc = b_mn_major ? cvh::encode_tmap_2d_bf16(&tmB, B, K, N, ldb, BK, 64)
                     : cvh::encode_tmap_2d_bf16(&tmB, B, N, K, ldb, 128, BK);   // 128-row boxes: BN / 128 per stage
     if (rc) return rc;
-    // C (and the pre-activation copy) as [32-row x 128-byte] boxes for the epilogue's TMA stores
-    alignas(64) CUtensorMap tmC, tmC2;
-    p.tma_store = !(p.dbg & 8);
-    if (p.tma_store) {
-        rc = c_is_f32 ? cvh::encode_tmap_2d_f32(&tmC, Cout, M, N, ldc, 32, 32) : cvh::encode_tmap_2d_bf16(&tmC, Cout, M, N, ldc, 32, 64);
-        if (rc) return rc;
-        tmC2 = tmC;
-        if (p.has_c2) {
-            rc = cvh::encode_tmap_2d_bf16(&tmC2, C2, M, N, ldc, 32, 64);
-            if (rc) return rc;
-        }
-    } else {
-        tmC = tmA;
-        tmC2 = tmA;
-    }
-    if (BN == 256) return dispatch<256>(a_mn_major, b_mn_major, c_is_f32, tmA, tmB, tmC, tmC2, p, s);
-    return dispatch<128>(a_mn_major, b_mn_major, c_is_f32, tmA, tmB, tmC, tmC2, p, s);
+    if (BN == 256) return dispatch<256>(a_mn_major, b_mn_major, c_is_f32, tmA, tmB, p, s);
+    return dispatch<128>(a_mn_major, b_mn_major, c_is_f32, tmA, tmB, p, s);
 }
 
 extern "C" int cv_gemm_bf16(const void* A, int a_mn_major, int64_t lda, const void* B, int b_mn_major, int64_t ldb,

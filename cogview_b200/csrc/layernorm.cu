@@ -101,8 +101,8 @@ ln_fwd_kernel(const TIn* __restrict__ x, const float* __restrict__ absmax_in, co
 }
 
 // Same operation with the row held in REGISTERS (cols <= 128 * NV): a lane issues all NV 16-byte loads of its row
-// before the first use, so 16 resident warps keep ~160 KB in flight per SM — the shared-memory staged kernel above has a
-// few loads in flight per warp and ran at 3.5 TB/s (111 MB in 31.4 us at the 4B shape, profiles/r01_train_step_launches_v3).
+// before the first use, so 16 resident warps keep ~160 KB in flight per SM — the shared-memory staged kernel above has
+// only a few loads in flight per warp.
 template <typename TIn, typename TOut, bool RES, int NV>
 __global__ void __launch_bounds__(WARPS * 32, 2)
 ln_fwd_reg_kernel(const TIn* __restrict__ x, const float* __restrict__ absmax_in, const __nv_bfloat16* __restrict__ gamma,
@@ -402,7 +402,7 @@ extern "C" int cv_layernorm_absmax_fwd(const void* x, int x_is_bf16, const float
         const char* e = getenv("COGVIEW_B200_LN_REG");
         reg_rows = (e && e[0] == '0') ? 0 : 1;
     }
-    // measured at 4352 x 2560: 19.9 vs 21.5 us without the residual, 37.8 vs 33.7 us with it (tools/ln_time.py)
+    // the register kernel serves rows without a residual; with one, the staged kernel is used (tools/ln_time.py times both)
     const bool use_reg = reg_rows && cols <= 128 * 20 && residual == nullptr;
     int rgrid = 2 * cvh::num_sms();                      // two CTAs of 8 warps per SM, rows grid-strided
     if (rgrid > (rows + WARPS - 1) / WARPS) rgrid = (rows + WARPS - 1) / WARPS;

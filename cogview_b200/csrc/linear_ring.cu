@@ -4,10 +4,9 @@
 // from the sampling loop (generation/sampling.py:147-151).  Same contract as linear_small_m_kernel (csrc/decode.cu);
 // cv_linear_small_m picks this kernel when the shape allows it.
 //
-// Why a second kernel: the fragment-direct loads of linear_small_m_kernel read HBM in 64-byte pieces through the LSU
-// and top out at 2.85 TB/s (profiles/r01_ncu_full_linear_small_m_v3_summary.txt); bulk copies of whole row segments
-// into a shared-memory ring stream at 6.5 TB/s (tools/micro/stream_bench.cu).  The machinery is the one the persistent
-// step kernel (csrc/decode_step.cu) was built and measured on:
+// Why a second kernel: the fragment-direct loads of linear_small_m_kernel read HBM in 64-byte pieces through the LSU;
+// bulk copies of whole row segments into a shared-memory ring keep more bytes in flight per SM.  The machinery is the
+// one the persistent step kernel (csrc/decode_step.cu) is built on:
 //   * 2 CTAs per SM, each owning a contiguous row range of W; per CTA 8 consumer warps + 1 producer warp + 1
 //     epilogue warp, ~100 KB of shared memory — small enough for the NEXT linear of the step to become resident
 //     (programmatic dependent launch) and start streaming ITS weights while this one finishes: weights never depend

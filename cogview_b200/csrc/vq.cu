@@ -164,7 +164,7 @@ __global__ void im2col_k4s2_c3_kernel(const float* __restrict__ img, __nv_bfloat
 // 8 lanes per pixel, 4 pixels per warp: lane `sub` owns channels 8 sub + 64 j + t (t < 8), so the 8 lanes of a pixel read
 // 128 contiguous bytes per step and up to 8 steps (1 KB per pixel at cin = 512) are in flight per lane; the 3 x cin weights
 // sit in shared memory.  (The first version gave a whole warp to ONE pixel at a time — 15 shuffles and 2 loads per pixel —
-// and ran at 0.72 TB/s: 1.5 ms per 16 images, a third of the VQ-VAE round trip; profiles/r02_ncu_full_vqvae_summary.txt.)
+// and kept too few loads in flight to approach the HBM bandwidth.)
 constexpr int C1_MAXJ = 8;      // cin <= 512 in one pass; larger cin loops
 __global__ void __launch_bounds__(256)
 conv1x1_out3_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ w, const float* __restrict__ bias,

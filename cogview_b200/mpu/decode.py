@@ -9,8 +9,7 @@ Two device paths:
   * COGVIEW_B200_PERSISTENT=1 and batch <= 8: the whole step — embedding, 48 Sandwich-LN layers, final LayerNorm,
     logits — is ONE persistent kernel (cv_decode_step, csrc/decode_step.cu: bulk-copy weight stream through a
     shared-memory byte ring, register-resident residual stream, grid barriers between the dependency points).  Parity-
-    green and profiled per phase (tools/step_prof.py), but at 63 us per layer against 59 us for the per-operation path
-    (4B, batch 4: 1289 vs 1411 tokens/s) it is not the default: DESIGN.md §5 has the anatomy.
+    green and profiled per phase (tools/step_prof.py); it is opt-in, the per-operation path is the default.
 """
 import os
 
@@ -45,7 +44,7 @@ class DecodeRunner:
         # enough (batch, head, split) CTAs to cover the SMs
         sms = torch.cuda.get_device_properties(dev).multi_processor_count
         # the key range of every (batch, head) is split so that ~8 CTAs per SM stream the K|V cache: the kernel is
-        # latency-bound per CTA (4B, b=4: 160 (batch, head) pairs alone left it at ~0.7 us per 16 keys)
+        # latency-bound per CTA, so one CTA per (batch, head) pair alone cannot fill the SMs
         self.nsplit = max(1, min(16, -(-8 * sms // (self.b * self.heads))))
         self.params = None
         self.param_sig = None

@@ -1,7 +1,7 @@
 """Parallel linears and embeddings — same classes, constructor signatures, parameter names/shapes and
 `.model_parallel` attributes as the reference's mpu/layers.py (VocabParallelEmbedding :77-133,
 ParallelEmbedding :136-182, ColumnParallelLinear :185-249, RowParallelLinear :252-326), with the
-model-parallel degree fixed at 1.  Forward and backward run on the tcgen05 GEMM (cv_gemm_bf16); the bias add
+model-parallel degree fixed at 1.  Forward and backward run on the wgmma GEMM (cv_gemm_bf16); the bias add
 (and, inside the transformer layer, GELU / abs-max) is fused in its epilogue."""
 import torch
 import torch.nn.init as init

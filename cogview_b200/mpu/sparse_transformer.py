@@ -1,5 +1,5 @@
 """Transformer stack — mirror of the reference's mpu/sparse_transformer.py: same class names, constructor
-signatures, parameter names (state_dict keys) and forward signatures, computed by the sm_100a kernels.
+signatures, parameter names (state_dict keys) and forward signatures, computed by the sm_90a kernels.
 
   LayerNorm                     :40-44    abs-max pre-scaled LN            -> cv_layernorm_absmax_*
   GPT2ParallelSelfAttention     :46-169   QKV GEMM, attention, out-proj    -> cv_gemm_bf16, cv_attn_*

@@ -1,4 +1,4 @@
-"""Fused AdamW for bf16 models with fp32 master weights — the B200 replacement of the reference's
+"""Fused AdamW for bf16 models with fp32 master weights — the CUDA replacement of the reference's
 FP16_Optimizer + apex FusedAdam + mpu.clip_grad_norm sequence (pretrain_gpt2.py:110-158, :380-389, :437-444;
 fp16/fp16.py:291-310, :399-453; mpu/grads.py:28-74).  bf16 needs no loss scaling, so the dynamic loss scaler
 disappears; the NaN/inf guard of train_step (pretrain_gpt2.py:415-417) stays with the caller.

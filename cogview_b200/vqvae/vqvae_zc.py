@@ -6,7 +6,7 @@ paths `encode` (img -> codes) and `decode_code` (codes -> img).  Training of the
 updates, gumbel relaxation, vqvae_zc.py:55-83, :284-346) is outside the accelerated path and raises.
 
 Device layout: NHWC bf16 activations; the three stride-2 4x4 convolutions and the three transposed convolutions run
-as im2col-free tcgen05 implicit GEMMs (cv_conv2d_k4s2 / cv_conv_transpose2d_k4s2), the Cin=3 first conv as
+as im2col-free wgmma implicit GEMMs (cv_conv2d_k4s2 / cv_conv_transpose2d_k4s2), the Cin=3 first conv as
 im2col + GEMM, the 1x1 convs as GEMMs, the quantiser as a 3-term bf16-split tensor-core GEMM + arg-min kernel."""
 import torch
 from torch import nn

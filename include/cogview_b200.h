@@ -1,5 +1,5 @@
 /*
- * cogview_b200.h — C ABI of libcogview_b200.so, the sm_100a implementation of CogView's hot path.
+ * cogview_b200.h — C ABI of libcogview_b200.so, the sm_90a (H100) implementation of CogView's hot path.
  *
  * The reference (THUDM/CogView) has no FFI: its operator boundary is the Python `mpu` / `model` /
  * `vqvae` namespaces.  Each entry point below replaces the torch/apex/cuBLAS call sequence of one
@@ -33,7 +33,7 @@ long long cv_launch_count(void);
 int cv_set_reserved_sms(int k);
 
 /* ------------------------------------------------------------------------------------------------
- * GEMM  C[M,N] = op(A)[M,K] * op(B)[N,K]^T (+ bias[N]) (+ tanh-GELU)      tcgen05 + TMA + TMEM
+ * GEMM  C[M,N] = op(A)[M,K] * op(B)[N,K]^T (+ bias[N]) (+ tanh-GELU)      wgmma + TMA
  *   replaces F.linear in ColumnParallelLinear.forward (mpu/layers.py:239-249),
  *   RowParallelLinear.forward (mpu/layers.py:312-326), gelu_impl (mpu/sparse_transformer.py:172-176),
  *   the tied-weight logits GEMM (model/gpt2_modeling.py:117-118) and their autograd backward.
@@ -147,7 +147,7 @@ int cv_colsum_bf16(const void* dy, int64_t ld, void* out, float* workspace, int 
  * pivot mask of :491-496 / :569 in closed form.  One softmax over
  *     band   : keys j with band_start(i) <= j <= i,  band_start(i) = max(0, i / w - times + 1) * w
  *     pivots : the n_piv gathered keys K[pivot_idx], V[pivot_idx] whose position is < band_start(i), scores + log(s / n_piv)
- * walked by ONE flash kernel as band tiles followed by gathered-pivot tiles (tcgen05 + TMA, same kernel as cv_attn_fwd);
+ * walked by ONE flash kernel as band tiles followed by gathered-pivot tiles (wgmma + TMA, same kernel as cv_attn_fwd);
  * masked entries carry exactly -10000 as in the reference.  q / k / v: [b, s, heads*64] bf16 views as for cv_attn_fwd;
  * pivot_idx: int64 [b, n_piv] (distinct positions per sequence, mpu/sparse_transformer.py:557-565); s % w == 0.
  * The backward runs the band pass and the pivot pass with the joint lse / delta, scatters the pivot dK / dV back and
@@ -304,7 +304,7 @@ int cv_clip_coef(const float* sumsq, float max_norm, float* coef, float* norm_ou
 /* ------------------------------------------------------------------------------------------------
  * VQ-VAE image tokenizer (vqvae/vqvae_zc.py, vqvae/api.py), NHWC bf16 activations.
  *   cv_conv2d_k4s2 / cv_conv_transpose2d_k4s2: nn.Conv2d / nn.ConvTranspose2d (kernel 4, stride 2, padding 1) of
- *     Encoder (vqvae_zc.py:121-129) and Decoder (:172-191) as im2col-free implicit GEMMs on tcgen05: A tiles are
+ *     Encoder (vqvae_zc.py:121-129) and Decoder (:172-191) as im2col-free implicit GEMMs on wgmma: A tiles are
  *     TMA boxes of the NHWC input (traversal stride 2 / sub-pixel phases, zero-filled halo = padding).
  *     x: [B, IH, IW, Cin]; w_packed: [16 (ky*4+kx), Cout, Cin] bf16; bias bf16 [Cout] or NULL; relu fused.
  *     y: [B, IH/2, IW/2, Cout] (conv) or [B, 2IH, 2IW, Cout] (transposed).  Cin % 64 == 0, Cout % 128 == 0,

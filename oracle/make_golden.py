@@ -22,7 +22,7 @@ from oracle import cogview_oracle as O  # noqa: E402
 from oracle import recipes, ref_harness  # noqa: E402
 
 GOLD = os.path.join(ROOT, "tests", "golden")
-VOCAB_STRIDE = 97  # logits are stored on every 97th vocab column (+ arg-max / top-8 per position)
+VOCAB_STRIDE = 194  # logits are stored on every 194th vocab column (+ arg-max / top-8 per position)
 
 
 def close(a, b, tol, what):

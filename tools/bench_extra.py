@@ -1,7 +1,7 @@
 """Measurements that are claimed in DESIGN.md but are not part of bench.py's headline line:
 
   sweep     : SURVEY §8(d) config 2 batch sweep — AR sampling tokens/s of the 4B model at b = 1, 4, 8 (persistent
-              one-kernel step), 16 (per-operation decode kernels, cv_linear_small_m M <= 16) and 64 (general tcgen05
+              one-kernel step), 16 (per-operation decode kernels, cv_linear_small_m M <= 16) and 64 (general wgmma
               GEMM path with the K|V cache)
   sr_dense  : BASELINE configs[4] as the reference SHIPS it (scripts/super_resolution.sh:7,36): dense attention,
               1345 positions — context 321 tokens, 1024 generated, 4 beams

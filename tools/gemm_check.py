@@ -1,4 +1,4 @@
-"""Bring-up check for cv_gemm_bf16 on a real B200: every operand-major combination, tile width and
+"""Bring-up check for cv_gemm_bf16 on a real H100: every operand-major combination, tile width and
 epilogue, each case in its own subprocess (a trap poisons the CUDA context) under a timeout.
 
     python tools/gemm_check.py            # run all cases, write gpurun_out/gemm_check.json

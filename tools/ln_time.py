@@ -1,7 +1,7 @@
 """LayerNorm kernels at the 4B layer shape (4352 x 2560): time and achieved HBM bandwidth.
 
     python tools/ln_time.py            (COGVIEW_B200_LN_REG=0 selects the shared-memory staged forward kernel)
-The inputs (2 x 45 MB) are rotated over 4 copies so that successive launches do not hit in the 126 MB L2."""
+The inputs (2 x 45 MB) are rotated over 4 copies so that successive launches do not hit in the 50 MB L2."""
 import os
 import sys
 

@@ -86,9 +86,9 @@ int main() {
     const int modes[] = {0, 1, 2, 3, 4, 5, 8, 12};
     for (int i = 0; i < 8; ++i) {
         cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
-        consume_kernel<<<148, 544, smem>>>(100, modes[i], out);
+        consume_kernel<<<132, 544, smem>>>(100, modes[i], out);
         cudaEventRecord(e0);
-        consume_kernel<<<148, 544, smem>>>(tiles, modes[i], out);
+        consume_kernel<<<132, 544, smem>>>(tiles, modes[i], out);
         cudaEventRecord(e1);
         cudaError_t err = cudaDeviceSynchronize();
         float ms; cudaEventElapsedTime(&ms, e0, e1);

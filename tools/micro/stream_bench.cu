@@ -1,6 +1,6 @@
-// Micro-benchmark: how fast can 148 persistent CTAs stream a big buffer through a shared-memory ring with
+// Micro-benchmark: how fast can one persistent CTA per SM stream a big buffer through a shared-memory ring with
 // cp.async.bulk row copies?  Variants: bytes per copy, smem row pitch, stages, consumer work.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o stream_bench stream_bench.cu && ./stream_bench
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o stream_bench stream_bench.cu && ./stream_bench
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>

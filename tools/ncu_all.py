@@ -1,4 +1,4 @@
-"""One profiled pass over every kernel family of the path, for `ncu --set full` (profiles/r02_ncu_*).
+"""One profiled pass over every kernel family of the path, for `ncu --set full`.
 
     ncu --set full --clock-control none --import-source on --profile-from-start off -o gpurun_out/r02_<group> \
         python tools/ncu_all.py <group>
@@ -7,7 +7,7 @@ groups:  train   GEMM (qkv shape), attention fwd / bwd (dense with dropout, spar
                  cross-entropy fwd / bwd, colsum, multi-tensor sum-of-squares + AdamW (a 4-layer model's parameters)
          decode  small-M linear (qkv shape, M = 4 and 16), ring linear, Sandwich-LN glue, cached attention, gathered (sparse) attention,
                  sampling epilogue, the persistent one-kernel step (4 layers)
-         vqvae   conv / transposed conv (tcgen05 implicit GEMM), im2col, split + distance GEMM + arg-min + lookup, 1x1-to-RGB
+         vqvae   conv / transposed conv (wgmma implicit GEMM), im2col, split + distance GEMM + arg-min + lookup, 1x1-to-RGB
 Each kernel runs twice untimed first; inputs are larger than L2 or the L2 is flushed before the profiled launch."""
 import os
 import sys
