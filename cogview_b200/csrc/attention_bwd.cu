@@ -17,6 +17,7 @@
 //   dK  += dS^T Q     (A = dS^T from registers, B = Q  MN-major)
 //   dQ_i = dS K       (A = dS^T of both warpgroups, written to smem and read MN-major, B = K MN-major)
 // dV / dK stay in registers for the whole loop; dQ tiles are reduced into an fp32 buffer with vector red.add.
+#include "attention_sparse.cuh"
 #include "common.cuh"
 #include "host.h"
 #include "../../include/cogview_b200.h"
@@ -43,8 +44,11 @@ struct BwdParams {
     const float* delta;  // [b, heads, s]
     float* dq_acc;       // [b, s, heads*HD] fp32, zero-initialised
     __nv_bfloat16* dqkv; // [b, s, 3*heads*HD]
-    const uint32_t* drop_mask;  // keep bits written by the forward, key-major ([b, heads, nkb*128, nqb, 4]: the 128 query
-                                // bits of (key, query block) are one 16-byte load for the thread that owns the key) or null
+    const uint32_t* drop_mask;  // keep bits written by the forward, key-major ([b, heads, keep_rows, keep_slots, 4]: the 128
+                                // query bits of (key, query tile) are one 16-byte load for the thread that owns the key) or
+                                // null.  Dense: keep_rows = nqb*128, slot = query block; sparse: the band / pivot region of
+                                // sparse::KeepLayout, slot = local query-tile counter t
+    int keep_rows, keep_slots;
     float drop_scale;           // 1 / (1 - p)
     // sparse training attention (mpu/sparse_transformer.py:675-725), two launches that share lse / delta / dq_acc:
     //   MODE_BAND : keys = the sequence, key j visible to query i iff band_start(i) <= j <= i
@@ -55,10 +59,7 @@ struct BwdParams {
     float piv_bias_log2;
 };
 
-__device__ __forceinline__ int band_start(int i, int w, int times) {
-    const int g = i / w - times + 1;
-    return g > 0 ? g * w : 0;
-}
+using sparse::band_start;
 
 __device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
     asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
@@ -88,9 +89,9 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     int i_start = (k0 < p.sep_eff) ? 0 : kb, i_end = nqb - 1;
     if (MODE == MODE_BAND) {          // queries i with band_start(i) <= j <= i
         i_start = kb;
-        i_end = min(nqb - 1, (((k0 + BLK - 1) / p.sp_w + p.sp_times) * p.sp_w - 1) / BLK);
+        i_end = sparse::bwd_band_last(kb, nqb, p.sp_w, p.sp_times);
     } else if (MODE == MODE_PIVOT) {  // band_start(i) > 0  <=>  i >= sp_times * sp_w   (the host checks this is < s)
-        i_start = (p.sp_times * p.sp_w) / BLK;
+        i_start = sparse::piv_first(p.sp_w, p.sp_times);
     }
     const int ntiles = i_end - i_start + 1;
 
@@ -135,7 +136,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
             my_pos[h] = (MODE == MODE_PIVOT) ? (kj[h] < p.sk ? p.piv_pos[(size_t)batch * p.sk + kj[h]] : 0x7fffffff) : 0;
         }
         const size_t stat_base = ((size_t)batch * p.heads + head) * p.s;
-        const size_t keep_base = ((size_t)batch * p.heads + head) * (size_t)nqb * BLK;   // key rows are padded to blocks
+        const size_t keep_base = ((size_t)batch * p.heads + head) * (size_t)p.keep_rows;   // key rows are padded to blocks
+        const int keep_slot0 = MODE == MODE_DENSE ? i_start : 0;
         const uint32_t k_addr = smem_u32(sK), v_addr = smem_u32(sV);
         const uint32_t kh_addr = k_addr + half * (64 * 128), vh_addr = v_addr + half * (64 * 128);
         float dv[HD / 2], dk[HD / 2];
@@ -159,7 +161,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
             if (use_drop) {
 #pragma unroll
                 for (int h = 0; h < 2; ++h)
-                    kw[h] = *reinterpret_cast<const uint4*>(p.drop_mask + ((keep_base + kj[h]) * (size_t)nqb + i_start + t) * 4);
+                    kw[h] = *reinterpret_cast<const uint4*>(p.drop_mask +
+                                                            ((keep_base + kj[h]) * (size_t)p.keep_slots + keep_slot0 + t) * 4);
             }
             named_bar_sync(1 + half, 128);
             mbar_wait<false>(&qdo_full[stage], phase);
@@ -383,6 +386,8 @@ extern "C" int cv_attn_bwd(const void* q, int64_t ldq, int64_t bsq, const void* 
     p.dqkv = static_cast<__nv_bfloat16*>(dqkv);
     p.drop_mask = dropout_p > 0.f ? drop_mask : nullptr;
     p.drop_scale = dropout_p > 0.f ? 1.0f / (1.0f - dropout_p) : 1.0f;
+    p.keep_rows = ((s + BLK - 1) / BLK) * BLK;
+    p.keep_slots = (s + BLK - 1) / BLK;
     p.sk = s; p.kv_rows = s; p.sp_w = 1; p.sp_times = 1; p.piv_pos = nullptr; p.piv_bias_log2 = 0.f;
     static bool attr_set = false;
     if (!attr_set) {
@@ -448,11 +453,14 @@ extern "C" int64_t cv_attn_sparse_bwd_workspace_bytes(int b, int heads, int head
                      al256b((size_t)b * n_piv * 3 * h * 2) + al256b((size_t)b * n_piv * 4));
 }
 
-extern "C" int cv_attn_sparse_bwd(const void* q, int64_t ldq, int64_t bsq, const void* k, int64_t ldk, int64_t bsk,
-                                  const void* v, int64_t ldv, int64_t bsv, const int64_t* pivot_idx, const void* out,
-                                  const void* d_out, const float* lse, void* dqkv, void* workspace, int b, int heads,
-                                  int head_dim, int s, int n_piv, int query_window, int key_window_times,
-                                  void* stream) {
+namespace {
+int attn_sparse_bwd(const void* q, int64_t ldq, int64_t bsq, const void* k, int64_t ldk, int64_t bsk, const void* v,
+                    int64_t ldv, int64_t bsv, const int64_t* pivot_idx, const void* out, const void* d_out,
+                    const float* lse, void* dqkv, void* workspace, int b, int heads, int head_dim, int s, int n_piv,
+                    int query_window, int key_window_times, float dropout_p, const uint32_t* drop_mask,
+                    cudaStream_t st) {
+    CV_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, "dropout probability must be in [0, 1)");
+    CV_REQUIRE(dropout_p == 0.f || drop_mask != nullptr, "attention dropout needs the keep mask saved by the forward");
     CV_REQUIRE(q && k && v && pivot_idx && out && d_out && lse && dqkv && workspace, "null pointer");
     CV_REQUIRE(head_dim == HD, "head_dim must be 64");
     CV_REQUIRE(b > 0 && heads > 0 && s > 0 && n_piv > 0 && n_piv <= s, "bad sizes");
@@ -460,7 +468,6 @@ extern "C" int cv_attn_sparse_bwd(const void* q, int64_t ldq, int64_t bsq, const
                "the sequence length must be a multiple of query_window");
     CV_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && bsq % 8 == 0 && bsk % 8 == 0 && bsv % 8 == 0,
                "strides must be multiples of 8 elements");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int h = heads * HD;
     char* ws = static_cast<char*>(workspace);
     float* dq_acc = reinterpret_cast<float*>(ws);
@@ -498,7 +505,8 @@ extern "C" int cv_attn_sparse_bwd(const void* q, int64_t ldq, int64_t bsq, const
     p.scale = 1.0f / sqrtf((float)head_dim);
     p.scale_log2 = p.scale * LOG2E;
     p.lse = lse; p.delta = delta; p.dq_acc = dq_acc;
-    p.drop_mask = nullptr; p.drop_scale = 1.0f;
+    p.drop_scale = dropout_p > 0.f ? 1.0f / (1.0f - dropout_p) : 1.0f;
+    const sparse::KeepLayout L = sparse::keep_layout(b, heads, s, n_piv, query_window, key_window_times);
     p.sp_w = query_window; p.sp_times = key_window_times;
     p.piv_bias_log2 = logf((float)(s / n_piv)) * LOG2E;
     static bool attr_set = false;
@@ -510,11 +518,15 @@ extern "C" int cv_attn_sparse_bwd(const void* q, int64_t ldq, int64_t bsq, const
     // band pass: dK / dV rows of the sequence
     p.dqkv = static_cast<__nv_bfloat16*>(dqkv);
     p.sk = s; p.kv_rows = s; p.piv_pos = nullptr;
+    p.drop_mask = dropout_p > 0.f ? drop_mask + L.fwd_words : nullptr;
+    p.keep_rows = L.nkb * BLK; p.keep_slots = L.tq;
     attn_bwd_kernel<MODE_BAND><<<dim3((s + BLK - 1) / BLK, heads, b), NUM_THREADS, SMEM_BYTES, st>>>(tmQ, tmK, tmV, tmDO, p);
     CV_LAUNCH_CHECK();
     if (key_window_times * query_window < s) {       // some query sees pivots at all
         p.dqkv = dpiv;
         p.sk = n_piv; p.kv_rows = n_piv; p.piv_pos = pos32;
+        p.drop_mask = dropout_p > 0.f ? drop_mask + L.fwd_words + L.band_words : nullptr;
+        p.keep_rows = L.npb * BLK; p.keep_slots = L.np;
         attn_bwd_kernel<MODE_PIVOT><<<dim3((n_piv + BLK - 1) / BLK, heads, b), NUM_THREADS, SMEM_BYTES, st>>>(
             tmQ, tmPK, tmPV, tmDO, p);
         CV_LAUNCH_CHECK();
@@ -531,4 +543,26 @@ extern "C" int cv_attn_sparse_bwd(const void* q, int64_t ldq, int64_t bsq, const
         CV_LAUNCH_CHECK();
     }
     return 0;
+}
+}  // namespace
+
+extern "C" int cv_attn_sparse_bwd(const void* q, int64_t ldq, int64_t bsq, const void* k, int64_t ldk, int64_t bsk,
+                                  const void* v, int64_t ldv, int64_t bsv, const int64_t* pivot_idx, const void* out,
+                                  const void* d_out, const float* lse, void* dqkv, void* workspace, int b, int heads,
+                                  int head_dim, int s, int n_piv, int query_window, int key_window_times,
+                                  void* stream) {
+    return attn_sparse_bwd(q, ldq, bsq, k, ldk, bsk, v, ldv, bsv, pivot_idx, out, d_out, lse, dqkv, workspace, b, heads,
+                           head_dim, s, n_piv, query_window, key_window_times, 0.f, nullptr,
+                           static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int cv_attn_sparse_bwd_dropout(const void* q, int64_t ldq, int64_t bsq, const void* k, int64_t ldk,
+                                          int64_t bsk, const void* v, int64_t ldv, int64_t bsv, const int64_t* pivot_idx,
+                                          const void* out, const void* d_out, const float* lse, void* dqkv,
+                                          void* workspace, int b, int heads, int head_dim, int s, int n_piv,
+                                          int query_window, int key_window_times, float dropout_p,
+                                          const uint32_t* drop_mask, void* stream) {
+    return attn_sparse_bwd(q, ldq, bsq, k, ldk, bsk, v, ldv, bsv, pivot_idx, out, d_out, lse, dqkv, workspace, b, heads,
+                           head_dim, s, n_piv, query_window, key_window_times, dropout_p, drop_mask,
+                           static_cast<cudaStream_t>(stream));
 }

@@ -18,6 +18,7 @@
 //                   (the four threads of a quad share a pair of rows), P as bf16 registers straight into the A operand
 //                   of O += P V (m64n64k16).  The two warpgroups run independently, so the softmax of one overlaps
 //                   the MMAs of the other.
+#include "attention_sparse.cuh"
 #include "common.cuh"
 #include "host.h"
 #include "../../include/cogview_b200.h"
@@ -50,6 +51,9 @@ struct AttnParams {
                         //  [0] key-major [b, heads, nkb_all*128 (key), nqb_all, 4]: word w of (key, query block) holds
                         //      queries qb*128 + 32w .. +31 (what the backward consumes: one 16-byte load per key row)
                         //  [1] query-major [b, heads, nqb_all*128 (query), nkb_all, 4]: what this kernel consumes
+                        // (sparse: the three regions of sparse::KeepLayout, written by attn_sparse_dropout_mask_kernel)
+    const uint32_t* keep_q; // the query-major keep bits this kernel reads: [b, heads, nqb_all*128, keep_slots, 4]
+    int keep_slots;         // entries per query row: nkb_all (dense), or one per tile of the sparse tile walk
     int nkb_all;        // ceil(sk / 128)
     int nqb_all;        // ceil(sq / 128)
     // sparse training attention (mpu/sparse_transformer.py:675-725; sp_w = 0: dense).  One softmax over
@@ -61,10 +65,7 @@ struct AttnParams {
     float piv_bias_log2;    // log(s / n_piv) * log2(e)
 };
 
-__device__ __forceinline__ int band_start(int i, int w, int times) {
-    const int g = i / w - times + 1;
-    return g > 0 ? g * w : 0;
-}
+using sparse::band_start;
 
 template <bool DROPOUT, bool SPARSE>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
@@ -153,18 +154,25 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         const float masked_val = -10000.0f * LOG2E;
         const uint4* keep_row[2] = {nullptr, nullptr};
         if (DROPOUT) {
-            const size_t region = (size_t)p.b * p.heads * p.nkb_all * p.nqb_all * (BQ * 4);   // words per region
 #pragma unroll
             for (int h = 0; h < 2; ++h)
-                keep_row[h] = reinterpret_cast<const uint4*>(p.drop_mask + region) +
-                              (((size_t)batch * p.heads + head) * p.nqb_all * BQ + qi[h]) * p.nkb_all;
+                keep_row[h] = reinterpret_cast<const uint4*>(p.keep_q) +
+                              (((size_t)batch * p.heads + head) * p.nqb_all * BQ + qi[h]) * p.keep_slots;
         }
         const uint32_t q_addr = smem_u32(sQ) + half * (64 * 128);
         mbar_wait<false>(q_full, 0);
         int stage = 0; uint32_t phase = 0;
         for (int j = 0; j < nkb; ++j) {
-            uint4 kw[2] = {make_uint4(0u, 0u, 0u, 0u), make_uint4(0u, 0u, 0u, 0u)};
-            if (DROPOUT) { kw[0] = keep_row[0][j]; kw[1] = keep_row[1][j]; }
+            // keep bits of this thread's 32 keys of rows h = 0, 1: bit 8 (i & 3) + 2 (i >> 2) + e <-> key 8i + c_in + e
+            uint32_t kbits[2] = {0u, 0u};
+            if (DROPOUT) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const uint4 k4 = keep_row[h][j];
+                    kbits[h] = ((k4.x >> c_in) & 0x03030303u) | (((k4.y >> c_in) & 0x03030303u) << 2) |
+                               (((k4.z >> c_in) & 0x03030303u) << 4) | (((k4.w >> c_in) & 0x03030303u) << 6);
+                }
+            }
             const bool piv_tile = SPARSE && j >= nband;
             const int k0 = SPARSE ? (piv_tile ? (j - nband) * BKV : (jb0 + j) * BKV) : j * BKV;
             mbar_wait<false>(&kv_full[stage], phase);
@@ -177,14 +185,17 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
                 wgmma_ss_n128<0, 0>(s, make_smem_desc_sw128(q_addr + k * 32, 0, 1024),
                                     make_smem_desc_sw128(k_addr + k * 32, 0, 1024), k != 0 ? 1u : 0u);
             wgmma_commit();
-            int pos[SPARSE ? BKV / 4 : 1];              // positions of this thread's 32 gathered keys (pivot tiles)
+            // pivot tiles: bit 2i + e of pvis[h] = this thread's gathered key 8i + c_in + e is visible to row h
+            uint32_t pvis[2] = {0u, 0u};
             if (piv_tile) {
 #pragma unroll
                 for (int i = 0; i < BKV / 8; ++i)
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
                         const int pj = k0 + 8 * i + c_in + e;
-                        pos[2 * i + e] = pj < p.n_piv ? p.piv_pos[(size_t)batch * p.n_piv + pj] : 0x7fffffff;
+                        const int pp = pj < p.n_piv ? p.piv_pos[(size_t)batch * p.n_piv + pj] : 0x7fffffff;
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) pvis[h] |= (pp < bs_row[h] ? 1u : 0u) << (2 * i + e);
                     }
             }
             wgmma_wait<0>();
@@ -206,9 +217,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
                         if (full_vis) {
                             v = x * p.scale_log2;
                         } else if (piv_tile) {
-                            const int pp = pos[SPARSE ? 2 * i + e : 0];
-                            v = pp < bs_row[h] ? x * p.scale_log2 + p.piv_bias_log2 : masked_val;
-                            if (pp == 0x7fffffff) v = -INFINITY;   // beyond the pivot list
+                            v = ((pvis[h] >> (2 * i + e)) & 1u) ? x * p.scale_log2 + p.piv_bias_log2 : masked_val;
+                            if (kj >= p.n_piv) v = -INFINITY;      // beyond the pivot list
                         } else {
                             const bool vis = SPARSE ? (kj >= bs_row[h] && kj <= qi[h])
                                                     : ((kj < p.sep_eff) || (kj <= causal_lim[h]));
@@ -237,10 +247,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
                     psum[h] += __low2float(pb) + __high2float(pb);
                     if (DROPOUT) {   // dropout acts on the normalised probabilities: the row sum stays undropped; the
                                      // 1/(1-p) scale is applied once to the output row at the end
-                        const uint4 k4 = kw[h];
-                        const uint32_t word = (i >> 2) == 0 ? k4.x : ((i >> 2) == 1 ? k4.y : ((i >> 2) == 2 ? k4.z : k4.w));
-                        const int bit = 8 * (i & 3) + c_in;
-                        w = pack_bf16x2(((word >> bit) & 1u) ? e0 : 0.f, ((word >> (bit + 1)) & 1u) ? e1 : 0.f);
+                        const int bit = 8 * (i & 3) + 2 * (i >> 2);
+                        w = pack_bf16x2(((kbits[h] >> bit) & 1u) ? e0 : 0.f, ((kbits[h] >> (bit + 1)) & 1u) ? e1 : 0.f);
                     }
                     pk[2 * i + h] = w;
                 }
@@ -372,6 +380,8 @@ extern "C" int cv_attn_fwd(const void* q, int64_t ldq, int64_t bsq, const void* 
         p.drop_mask = drop_mask;
         p.nkb_all = (sk + BKV - 1) / BKV;
         p.nqb_all = (sq + BQ - 1) / BQ;
+        p.keep_q = drop_mask ? drop_mask + (size_t)b * heads * p.nkb_all * p.nqb_all * (BQ * 4) : nullptr;   // region [1]
+        p.keep_slots = p.nkb_all;
     }
     p.sp_w = 0; p.sp_times = 0; p.n_piv = 0; p.piv_pos = nullptr; p.piv_bias_log2 = 0.f;
     static bool attr_set = false;
@@ -412,6 +422,63 @@ __global__ void gather_pivots_kernel(const __nv_bfloat16* __restrict__ k, int64_
         d[h / 8 + i] = vs[i];
     }
 }
+
+// Keep decisions of the attention-probability dropout of the sparse attention, in the layout of sparse::KeepLayout.
+// The keys of query i are virtual: the s sequence positions (band keys), then the n_piv pivot SLOTS (pivot p is its own
+// key whatever its position, as column p of the reference's [b, heads, s, n_piv + w*times] probabilities).  One thread
+// per (query, virtual key tile) as in attn_dropout_mask_kernel: the Philox4x32-10 call of counter
+// ((batch*heads + head)*s + query) * (nkb + npb) + tile seeds four 32-step LCG streams, keep iff state >= p * 2^32.
+// A tile is written to the forward region and/or to the backward region of its pass when that kernel visits it.
+__global__ void __launch_bounds__(128, 4)
+attn_sparse_dropout_mask_kernel(const DropoutArgs drop, uint32_t* __restrict__ mask, const sparse::KeepLayout L,
+                                int heads, int s, int w, int times) {
+    const int qb = blockIdx.x, vb = blockIdx.y;
+    const int head = blockIdx.z % heads, batch = blockIdx.z / heads;
+    int fslot = -1, bslot = -1;            // entry of this tile in the forward / backward walk, -1: not visited
+    if (vb < L.nkb) {
+        const int jb0 = sparse::fwd_band_first(qb, w, times);
+        if (vb >= jb0 && vb < jb0 + sparse::fwd_band_count(qb, s, w, times)) fslot = vb - jb0;
+        if (qb >= vb && qb <= sparse::bwd_band_last(vb, L.nqb, w, times)) bslot = qb - vb;
+    } else {
+        if (sparse::fwd_sees_pivots(qb, s, w, times)) fslot = sparse::fwd_band_count(qb, s, w, times) + vb - L.nkb;
+        if (L.np > 0 && qb >= sparse::piv_first(w, times)) bslot = qb - sparse::piv_first(w, times);
+    }
+    if (fslot < 0 && bslot < 0) return;
+    const int lane = threadIdx.x & 31, wq = threadIdx.x >> 5;
+    const int qi = qb * BQ + threadIdx.x;
+    const size_t bh = (size_t)batch * heads + head;
+    const uint64_t ctr = ((uint64_t)bh * s + qi) * (uint64_t)(L.nkb + L.npb) + vb;
+    const uint4 r0 = philox4x32_10(drop.seed, ctr, drop.stream);
+    uint32_t rng[4] = {r0.x, r0.y, r0.z, r0.w};
+    uint32_t wrow[4], wkey[4];
+#pragma unroll
+    for (int g = 0; g < 4; ++g) {
+        uint32_t bits = 0u, mine = 0u;
+#pragma unroll
+        for (int t = 0; t < 32; ++t) {
+            rng[g] = rng[g] * 1664525u + 1013904223u;
+            const bool keep = rng[g] >= drop.threshold;
+            bits |= (keep ? 1u : 0u) << t;
+            const uint32_t bal = __ballot_sync(0xffffffffu, keep);   // key 32g + t over this warp's 32 queries
+            if (lane == t) mine = bal;
+        }
+        wrow[g] = bits;
+        wkey[g] = mine;
+    }
+    if (fslot >= 0)
+        reinterpret_cast<uint4*>(mask)[(bh * L.nqb * BQ + qi) * (L.tb + L.npb) + fslot] =
+            make_uint4(wrow[0], wrow[1], wrow[2], wrow[3]);
+    if (bslot >= 0) {
+        const bool band = vb < L.nkb;
+        const int slots = band ? L.tq : L.np;
+        const size_t rows = (size_t)(band ? L.nkb : L.npb) * BKV;        // key rows per (batch, head)
+        const int key0 = (band ? vb : vb - L.nkb) * BKV;
+        uint32_t* dm = mask + L.fwd_words + (band ? 0 : L.band_words) +
+                       ((bh * rows + key0 + lane) * slots + bslot) * 4 + wq;
+#pragma unroll
+        for (int g = 0; g < 4; ++g) dm[(size_t)g * 32 * slots * 4] = wkey[g];
+    }
+}
 }  // namespace
 
 extern "C" int64_t cv_attn_sparse_workspace_bytes(int b, int heads, int head_dim, int n_piv) {
@@ -419,11 +486,23 @@ extern "C" int64_t cv_attn_sparse_workspace_bytes(int b, int heads, int head_dim
     return ((int64_t)b * n_piv * 2 * h * 2 + 255) / 256 * 256 + (int64_t)b * n_piv * 4;
 }
 
-extern "C" int cv_attn_sparse_fwd(const void* q, int64_t ldq, int64_t bsq, const void* k, int64_t ldk, int64_t bsk,
-                                  const void* v, int64_t ldv, int64_t bsv, const int64_t* pivot_idx, void* out,
-                                  int64_t ldo, int64_t bso, float* lse, void* workspace, int b, int heads,
-                                  int head_dim, int s, int n_piv, int query_window, int key_window_times,
-                                  void* stream) {
+extern "C" int64_t cv_attn_sparse_drop_mask_words(int b, int heads, int s, int n_piv, int query_window,
+                                                  int key_window_times) {
+    CV_REQUIRE(b > 0 && heads > 0 && s > 0 && n_piv > 0 && n_piv <= s, "bad sizes");
+    CV_REQUIRE(query_window > 0 && key_window_times > 0 && s % query_window == 0,
+               "the sequence length must be a multiple of query_window");
+    const sparse::KeepLayout L = sparse::keep_layout(b, heads, s, n_piv, query_window, key_window_times);
+    return L.fwd_words + L.band_words + L.piv_words;
+}
+
+namespace {
+int attn_sparse_fwd(const void* q, int64_t ldq, int64_t bsq, const void* k, int64_t ldk, int64_t bsk, const void* v,
+                    int64_t ldv, int64_t bsv, const int64_t* pivot_idx, void* out, int64_t ldo, int64_t bso, float* lse,
+                    void* workspace, int b, int heads, int head_dim, int s, int n_piv, int query_window,
+                    int key_window_times, float dropout_p, uint64_t seed, uint32_t site, uint32_t* drop_mask,
+                    cudaStream_t st) {
+    CV_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, "dropout probability must be in [0, 1)");
+    CV_REQUIRE(dropout_p == 0.f || drop_mask != nullptr, "attention dropout needs the keep-mask buffer");
     CV_REQUIRE(q && k && v && pivot_idx && out && workspace, "null pointer");
     CV_REQUIRE(head_dim == HD, "head_dim must be 64 (CogView: hidden / heads = 64)");
     CV_REQUIRE(b > 0 && heads > 0 && s > 0 && n_piv > 0 && n_piv <= s, "bad sizes");
@@ -432,7 +511,6 @@ extern "C" int cv_attn_sparse_fwd(const void* q, int64_t ldq, int64_t bsq, const
     CV_REQUIRE(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0 && bsq % 8 == 0 && bsk % 8 == 0 &&
                    bsv % 8 == 0 && bso % 8 == 0,
                "strides must be multiples of 8 elements");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int h = heads * HD;
     __nv_bfloat16* pkv = static_cast<__nv_bfloat16*>(workspace);
     int* pos32 = reinterpret_cast<int*>(static_cast<char*>(workspace) + ((size_t)b * n_piv * 2 * h * 2 + 255) / 256 * 256);
@@ -453,19 +531,54 @@ extern "C" int cv_attn_sparse_fwd(const void* q, int64_t ldq, int64_t bsq, const
     p.scale_log2 = (1.0f / sqrtf((float)head_dim)) * LOG2E;
     p.out = static_cast<__nv_bfloat16*>(out);
     p.ldo = ldo; p.bso = bso; p.lse = lse;
-    p.drop.p = 0.f; p.drop.scale = 1.f; p.drop.threshold = 0; p.drop.stream = 0; p.drop.seed = 0;
-    p.drop_mask = nullptr;
+    const cvh::HostDropout hd = cvh::make_dropout(dropout_p, seed, site);
+    p.drop.p = hd.p; p.drop.scale = hd.scale; p.drop.threshold = hd.threshold; p.drop.stream = hd.stream;
+    p.drop.seed = hd.seed;
+    p.drop_mask = drop_mask;
     p.nkb_all = (s + BKV - 1) / BKV;
     p.nqb_all = (s + BQ - 1) / BQ;
     p.sp_w = query_window; p.sp_times = key_window_times; p.n_piv = n_piv; p.piv_pos = pos32;
     p.piv_bias_log2 = logf((float)(s / n_piv)) * LOG2E;           // integer division as in :697
+    const sparse::KeepLayout L = sparse::keep_layout(b, heads, s, n_piv, query_window, key_window_times);
+    p.keep_q = drop_mask;                                         // the forward region comes first
+    p.keep_slots = L.tb + L.npb;
     static bool attr_set = false;
     if (!attr_set) {
         CV_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+        CV_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
         attr_set = true;
     }
     dim3 grid((s + BQ - 1) / BQ, heads, b);
-    attn_fwd_kernel<false, true><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(tmQ, tmK, tmV, tmPK, tmPV, p);
+    if (dropout_p > 0.f) {
+        attn_sparse_dropout_mask_kernel<<<dim3(L.nqb, L.nkb + L.npb, b * heads), 128, 0, st>>>(
+            p.drop, drop_mask, L, heads, s, query_window, key_window_times);
+        CV_LAUNCH_CHECK();
+        attn_fwd_kernel<true, true><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(tmQ, tmK, tmV, tmPK, tmPV, p);
+    } else {
+        attn_fwd_kernel<false, true><<<grid, NUM_THREADS, SMEM_BYTES, st>>>(tmQ, tmK, tmV, tmPK, tmPV, p);
+    }
     CV_LAUNCH_CHECK();
     return 0;
+}
+}  // namespace
+
+extern "C" int cv_attn_sparse_fwd(const void* q, int64_t ldq, int64_t bsq, const void* k, int64_t ldk, int64_t bsk,
+                                  const void* v, int64_t ldv, int64_t bsv, const int64_t* pivot_idx, void* out,
+                                  int64_t ldo, int64_t bso, float* lse, void* workspace, int b, int heads,
+                                  int head_dim, int s, int n_piv, int query_window, int key_window_times,
+                                  void* stream) {
+    return attn_sparse_fwd(q, ldq, bsq, k, ldk, bsk, v, ldv, bsv, pivot_idx, out, ldo, bso, lse, workspace, b, heads,
+                           head_dim, s, n_piv, query_window, key_window_times, 0.f, 0, 0, nullptr,
+                           static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int cv_attn_sparse_fwd_dropout(const void* q, int64_t ldq, int64_t bsq, const void* k, int64_t ldk,
+                                          int64_t bsk, const void* v, int64_t ldv, int64_t bsv, const int64_t* pivot_idx,
+                                          void* out, int64_t ldo, int64_t bso, float* lse, void* workspace, int b,
+                                          int heads, int head_dim, int s, int n_piv, int query_window,
+                                          int key_window_times, float dropout_p, uint64_t seed, uint32_t site,
+                                          uint32_t* drop_mask, void* stream) {
+    return attn_sparse_fwd(q, ldq, bsq, k, ldk, bsk, v, ldv, bsv, pivot_idx, out, ldo, bso, lse, workspace, b, heads,
+                           head_dim, s, n_piv, query_window, key_window_times, dropout_p, seed, site, drop_mask,
+                           static_cast<cudaStream_t>(stream));
 }

@@ -151,7 +151,7 @@ int cv_colsum_bf16(const void* dy, int64_t ld, void* out, float* workspace, int 
  * masked entries carry exactly -10000 as in the reference.  q / k / v: [b, s, heads*64] bf16 views as for cv_attn_fwd;
  * pivot_idx: int64 [b, n_piv] (distinct positions per sequence, mpu/sparse_transformer.py:557-565); s % w == 0.
  * The backward runs the band pass and the pivot pass with the joint lse / delta, scatters the pivot dK / dV back and
- * writes dqkv [b, s, 3*heads*64] (dQ | dK | dV).  Attention-probability dropout is not available in this mode.
+ * writes dqkv [b, s, 3*heads*64] (dQ | dK | dV).
  * ---------------------------------------------------------------------------------------------- */
 int64_t cv_attn_sparse_workspace_bytes(int b, int heads, int head_dim, int n_piv);
 int cv_attn_sparse_fwd(const void* q, int64_t ldq, int64_t bsq, const void* k, int64_t ldk, int64_t bsk, const void* v,
@@ -163,6 +163,36 @@ int cv_attn_sparse_bwd(const void* q, int64_t ldq, int64_t bsq, const void* k, i
                        int64_t ldv, int64_t bsv, const int64_t* pivot_idx, const void* out, const void* d_out,
                        const float* lse, void* dqkv, void* workspace, int b, int heads, int head_dim, int s, int n_piv,
                        int query_window, int key_window_times, void* stream);
+/* The same with dropout on the joint pivot + band probabilities (attention_dropout of mpu/sparse_transformer.py:719-721):
+ * the row sum and lse stay undropped, the 1/(1-p) scale is applied once to the output row, and the backward sends dP and
+ * dV through the keep bits.  The keep decision of (query i, key) is a pure function of (seed, site, batch, head, i,
+ * virtual key), where the virtual keys are the s sequence positions (band keys) followed by the n_piv pivot SLOTS: pivot
+ * p is decided as column p of the reference's [b, heads, s, n_piv + w*times] probabilities, whatever its position.
+ * One Philox4x32-10 call of counter ((batch*heads + head)*s + i) * (nkb + npb) + virtual key tile seeds four 32-step
+ * LCG streams (key 32g + t of the tile is step t of stream g), keep iff state >= p * 2^32.
+ *   drop_mask: uint32 buffer of cv_attn_sparse_drop_mask_words() words, filled by the forward and read by the backward
+ *   (pass the same pointer), three regions in this order, with nqb = nkb = ceil(s/128), npb = ceil(n_piv/128):
+ *     [fwd]  query-major [b, heads, nqb*128 (query), TB + npb, 4]: bit t of word g of (query i, slot j) is key 32g + t of
+ *            the j-th tile query block i/128 visits: band key tiles jb0 .. jb0 + nband - 1 (jb0 = band_start(128 qb)/128,
+ *            nband = last query of the block / 128 - jb0 + 1), then, if band_start(last query) > 0, pivot tiles 0 .. npb-1
+ *            at slots nband .. nband + npb - 1.  TB = the largest nband.
+ *     [band] key-major [b, heads, nkb*128 (key), TQ, 4]: bit t of word g of (key, slot u) is query 128 (kb + u) + 32g + t,
+ *            kb = key / 128, for u = 0 .. i_end(kb) - kb, i_end(kb) = min(nqb - 1, ((((kb+1)*128 - 1) / w + times) * w - 1) / 128).
+ *            TQ = the largest i_end(kb) - kb + 1.
+ *     [piv]  key-major [b, heads, npb*128 (pivot slot), NP, 4]: bit t of word g of (pivot p, slot u) is query
+ *            128 (i0 + u) + 32g + t, i0 = (times*w) / 128; NP = nqb - i0 when times*w < s, else 0 (no query sees a pivot).
+ *   Entries that neither kernel reads are left unwritten. */
+int64_t cv_attn_sparse_drop_mask_words(int b, int heads, int s, int n_piv, int query_window, int key_window_times);
+int cv_attn_sparse_fwd_dropout(const void* q, int64_t ldq, int64_t bsq, const void* k, int64_t ldk, int64_t bsk,
+                               const void* v, int64_t ldv, int64_t bsv, const int64_t* pivot_idx, void* out, int64_t ldo,
+                               int64_t bso, float* lse, void* workspace, int b, int heads, int head_dim, int s, int n_piv,
+                               int query_window, int key_window_times, float dropout_p, uint64_t seed, uint32_t site,
+                               uint32_t* drop_mask, void* stream);
+int cv_attn_sparse_bwd_dropout(const void* q, int64_t ldq, int64_t bsq, const void* k, int64_t ldk, int64_t bsk,
+                               const void* v, int64_t ldv, int64_t bsv, const int64_t* pivot_idx, const void* out,
+                               const void* d_out, const float* lse, void* dqkv, void* workspace, int b, int heads,
+                               int head_dim, int s, int n_piv, int query_window, int key_window_times, float dropout_p,
+                               const uint32_t* drop_mask, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Decode (one new token per sequence): HBM-bound weight streaming, CUDA cores.
