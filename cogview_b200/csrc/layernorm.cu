@@ -172,11 +172,12 @@ ln_fwd_reg_kernel(const TIn* __restrict__ x, const float* __restrict__ absmax_in
 // Backward.  dy: gradient of the LN output (TDy); dres (optional fp32): gradient already flowing on the
 // residual path that must be added to dx (fp32 output) — used for the input/post-attention/final LNs.
 //   dx = rstd * (g*dy - mean(g*dy) - xhat * mean(g*dy*xhat)),  xhat = (x - mean) * rstd
+// drop.p > 0: x was the output of a dropout site, so dx is masked as in ln_bwd_fused_kernel (same element counter).
 template <typename TIn, typename TDy, typename TDx>
 __global__ void __launch_bounds__(WARPS * 32)
 ln_bwd_dx_kernel(const TIn* __restrict__ x, const TDy* __restrict__ dy, const float* __restrict__ mean_in,
                  const float* __restrict__ rstd_in, const __nv_bfloat16* __restrict__ gamma,
-                 const float* __restrict__ dres, TDx* __restrict__ dx, int rows, int cols) {
+                 const float* __restrict__ dres, TDx* __restrict__ dx, int rows, int cols, const DropoutArgs drop) {
     extern __shared__ float smem_f[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     float* sx = smem_f + (size_t)warp * 2 * cols;   // xhat
@@ -210,6 +211,7 @@ ln_bwd_dx_kernel(const TIn* __restrict__ x, const TDy* __restrict__ dy, const fl
                 float4 r = ld4(dres + (size_t)row * cols + i);
                 o.x += r.x; o.y += r.y; o.z += r.z; o.w += r.w;
             }
+            if (drop.p > 0.f) dropout4(drop, ((size_t)row * cols + i) >> 2, o.x, o.y, o.z, o.w);
             st4(dxr + i, o);
         }
         __syncwarp();
@@ -445,14 +447,9 @@ extern "C" int cv_layernorm_absmax_bwd(const void* x, int x_is_bf16, const void*
     const cvh::HostDropout hd = cvh::make_dropout(dropout_p, seed, site);
     DropoutArgs dargs;
     dargs.p = hd.p; dargs.scale = hd.scale; dargs.threshold = hd.threshold; dargs.stream = hd.stream; dargs.seed = hd.seed;
-    CV_REQUIRE(dropout_p == 0.f || (cols % 256 == 0 && cols / 8 <= 512),
-               "dropout in the LayerNorm backward needs the fused path (hidden size % 256 == 0)");
     CV_REQUIRE(x && dy && mean && rstd && gamma && dx && dgamma && dbeta && workspace, "null pointer");
     CV_REQUIRE(rows > 0 && cols > 0 && cols % 4 == 0, "cols must be a positive multiple of 4");
     cudaStream_t s = static_cast<cudaStream_t>(stream);
-    const size_t smem = (size_t)WARPS * 2 * cols * sizeof(float);
-    CV_REQUIRE(smem <= 220 * 1024, "hidden size too large for the row cache");
-    const int grid = fwd_grid(rows);
     const __nv_bfloat16* g = static_cast<const __nv_bfloat16*>(gamma);
     // fused path (parameter gradients in registers, every operand read once)
     if (cols % 256 == 0 && cols / 8 <= 512) {
@@ -481,6 +478,10 @@ extern "C" int cv_layernorm_absmax_bwd(const void* x, int x_is_bf16, const void*
         return 0;
     }
     CV_REQUIRE(dxsum == nullptr, "the column sum of dx is only produced by the fused path (hidden size % 256 == 0)");
+    // the unfused dx kernel stages two fp32 rows per warp in shared memory
+    const size_t smem = (size_t)WARPS * 2 * cols * sizeof(float);
+    CV_REQUIRE(smem <= 220 * 1024, "hidden size too large for the row cache");
+    const int grid = fwd_grid(rows);
     const int splits = rows < PARAM_ROW_SPLITS ? rows : PARAM_ROW_SPLITS;
     dim3 pgrid((cols + 127) / 128, splits);
 #define LAUNCH(TI, TDY, TDX)                                                                                   \
@@ -488,7 +489,7 @@ extern "C" int cv_layernorm_absmax_bwd(const void* x, int x_is_bf16, const void*
         auto k = ln_bwd_dx_kernel<TI, TDY, TDX>;                                                               \
         CV_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));              \
         k<<<grid, WARPS * 32, smem, s>>>(static_cast<const TI*>(x), static_cast<const TDY*>(dy), mean, rstd, g, \
-                                         dres, static_cast<TDX*>(dx), rows, cols);                             \
+                                         dres, static_cast<TDX*>(dx), rows, cols, dargs);                      \
         ln_bwd_param_kernel<TI, TDY><<<pgrid, 128, 0, s>>>(static_cast<const TI*>(x), static_cast<const TDY*>(dy), \
                                                            mean, rstd, workspace, rows, cols);                  \
     } while (0)

@@ -53,22 +53,42 @@ __global__ void embed_fwd_kernel(const int64_t* __restrict__ ids, const int64_t*
     }
 }
 
-// dwte[ids[r]] += dx[r], dwpe[pos[r]] += dx[r]  (bf16 gradients, bf16x2 atomics)
+// dwte[ids[r]] += dx[r], dwpe[pos[r]] += dx[r]  (bf16 gradients).  One warp per task = (table, row r); the task whose
+// row is the first one carrying its index adds every row carrying that index, in row order, and the others do nothing.
+// A token or position that occurs three or more times thus gets the same gradient bits on every run (atomics would add
+// in arrival order).
 __global__ void embed_bwd_kernel(const int64_t* __restrict__ ids, const int64_t* __restrict__ pos,
                                  const float* __restrict__ dx, __nv_bfloat16* __restrict__ dwte,
                                  __nv_bfloat16* __restrict__ dwpe, int rows, int h, const DropoutArgs drop) {
     const int warps_per_block = blockDim.x >> 5;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    for (int r = blockIdx.x * warps_per_block + warp; r < rows; r += gridDim.x * warps_per_block) {
-        __nv_bfloat162* a = reinterpret_cast<__nv_bfloat162*>(dwte + (size_t)ids[r] * h);
-        __nv_bfloat162* b = reinterpret_cast<__nv_bfloat162*>(dwpe + (size_t)pos[r] * h);
-        const float4* d = reinterpret_cast<const float4*>(dx + (size_t)r * h);
-        for (int i = lane; i < h / 4; i += 32) {
-            float4 v = d[i];
-            if (drop.p > 0.f) dropout4(drop, ((uint64_t)r * h + 4 * (uint64_t)i) >> 2, v.x, v.y, v.z, v.w);
-            const __nv_bfloat162 b0 = __floats2bfloat162_rn(v.x, v.y), b1 = __floats2bfloat162_rn(v.z, v.w);
-            atomicAdd(a + 2 * i, b0); atomicAdd(a + 2 * i + 1, b1);
-            atomicAdd(b + 2 * i, b0); atomicAdd(b + 2 * i + 1, b1);
+    for (int task = blockIdx.x * warps_per_block + warp; task < 2 * rows; task += gridDim.x * warps_per_block) {
+        const bool is_pos = task >= rows;
+        const int r = is_pos ? task - rows : task;
+        const int64_t* idx = is_pos ? pos : ids;
+        const int64_t v = idx[r];
+        bool seen = false;
+        for (int j0 = 0; j0 < r && !seen; j0 += 32) seen = __any_sync(0xffffffffu, j0 + lane < r && idx[j0 + lane] == v);
+        if (seen) continue;
+        __nv_bfloat162* o = reinterpret_cast<__nv_bfloat162*>((is_pos ? dwpe : dwte) + (size_t)v * h);
+        for (int j0 = r; j0 < rows; j0 += 32) {
+            unsigned m = __ballot_sync(0xffffffffu, j0 + lane < rows && idx[j0 + lane] == v);
+            while (m) {
+                const int j = j0 + __ffs(m) - 1;
+                m &= m - 1;
+                const float4* d = reinterpret_cast<const float4*>(dx + (size_t)j * h);
+                for (int i = lane; i < h / 4; i += 32) {
+                    float4 x = d[i];
+                    if (drop.p > 0.f) dropout4(drop, ((uint64_t)j * h + 4 * (uint64_t)i) >> 2, x.x, x.y, x.z, x.w);
+                    // dx is rounded to bf16 before the add, and the sum rounded again, as a bf16 atomicAdd does: a
+                    // row that occurs once or twice gets exactly the bits it got from atomics
+                    const float2 a = __bfloat1622float2(o[2 * i]), b = __bfloat1622float2(o[2 * i + 1]);
+                    const float2 p = __bfloat1622float2(__floats2bfloat162_rn(x.x, x.y));
+                    const float2 q = __bfloat1622float2(__floats2bfloat162_rn(x.z, x.w));
+                    o[2 * i] = __floats2bfloat162_rn(a.x + p.x, a.y + p.y);
+                    o[2 * i + 1] = __floats2bfloat162_rn(b.x + q.x, b.y + q.y);
+                }
+            }
         }
     }
 }
@@ -294,7 +314,7 @@ extern "C" int cv_embed_bwd(const int64_t* ids, const int64_t* pos, const float*
     CV_REQUIRE(ids && pos && dx && dwte && dwpe, "null pointer");
     CV_REQUIRE(rows > 0 && hidden > 0 && hidden % 4 == 0, "hidden must be a multiple of 4");
     const int wpb = 8;
-    int blocks = (rows + wpb - 1) / wpb;
+    int blocks = (2 * rows + wpb - 1) / wpb;
     int cap = cvh::num_sms() * 4;
     embed_bwd_kernel<<<blocks < cap ? blocks : cap, wpb * 32, 0, static_cast<cudaStream_t>(stream)>>>(
         ids, pos, dx, static_cast<__nv_bfloat16*>(dwte), static_cast<__nv_bfloat16*>(dwpe), rows, hidden,

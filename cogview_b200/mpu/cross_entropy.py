@@ -15,7 +15,11 @@ class _VocabParallelCrossEntropy(torch.autograd.Function):
         if logits.dtype != torch.float32:
             logits = logits.float()
         if logits.stride(1) != 1 or logits.stride(0) % 4 != 0:
-            logits = logits.contiguous()
+            # the kernels read rows at a stride that is a multiple of 4: copy into a row-padded buffer
+            # (.contiguous() would keep stride V for an odd vocabulary)
+            buf = torch.empty((logits.shape[0], (V + 3) // 4 * 4), dtype=torch.float32, device=logits.device)
+            buf[:, :V].copy_(logits)
+            logits = buf[:, :V]
         loss, rmax, rsum = ops.cross_entropy_fwd(logits, target.reshape(-1))
         ctx.save_for_backward(logits, target.reshape(-1), rmax, rsum)
         ctx.in_dtype = vocab_parallel_logits.dtype
