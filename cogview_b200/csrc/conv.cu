@@ -7,6 +7,11 @@
 // tap is one TMA box of the NHWC input — [64 channels x TW x TH x NB] with traversal stride 2 in W and H for the
 // strided convolution (elementStrides), out-of-bounds coordinates zero-filled by TMA (that IS the padding) — so
 // no im2col buffer is ever materialised.  Weights are pre-packed [tap][Cout][Cin] (K-major B tiles).
+// Tile shapes over the [B, H, W] grid of tile pixels (output grid for the strided conv, input grid for a phase):
+//   W <= 128, H and W powers of two: whole rows, TW = W, TH = 128 / W (NB = 1), or whole images (NB = 128 / (H W));
+//   W > 128, W % 128 == 0, any H:    row segments, TW = 128, TH = NB = 1 (one tile = columns x0 .. x0+127 of
+//                                    one row; a TMA box extent is at most 256, so the strided conv's 2 TW and a
+//                                    phase's TW cannot cover a wider row).
 // The transposed convolution is computed as its 4 sub-pixel phases (each a 2x2-tap stride-1 convolution on the
 // input grid); a phase's output pixels are scattered to (2a+py, 2b+px).
 // Pipeline and warpgroup roles are those of gemm.cu; epilogue = bias (+ReLU) -> bf16 -> global stores.
@@ -33,8 +38,9 @@ struct Cfg {
 struct ConvParams {
     int Cin, Cout;
     int H, W;            // tile grid: output dims for the strided conv, input dims for a transposed-conv phase
-    int TH, NB;          // tile = NB images x TH rows x W columns = 128 pixels
+    int TH, NB;          // tile = NB images x TH rows x W columns = 128 pixels (W <= 128)
     int tiles_per_image; // (H*W)/128 when >= 1 (then NB == 1)
+    int row_segs;        // W > 128: tiles per row (W / 128; TH = NB = 1); 0 when tiles span whole rows
     int num_m_tiles, num_n_blocks, kc_blocks, ntaps;
     int py, px;          // transposed conv: output phase
     const __nv_bfloat16* bias;
@@ -70,8 +76,12 @@ conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     }
     __syncthreads();
 
-    auto tile_origin = [&](int mt, int& b0, int& y0) {
-        if (p.tiles_per_image >= 1) { b0 = mt / p.tiles_per_image; y0 = (mt % p.tiles_per_image) * p.TH; }
+    auto tile_origin = [&](int mt, int& b0, int& y0, int& x0) {
+        x0 = 0;
+        if (p.row_segs > 0) {
+            const int t = mt % p.tiles_per_image;
+            b0 = mt / p.tiles_per_image; y0 = t / p.row_segs; x0 = (t % p.row_segs) * BM;
+        } else if (p.tiles_per_image >= 1) { b0 = mt / p.tiles_per_image; y0 = (mt % p.tiles_per_image) * p.TH; }
         else { b0 = mt * p.NB; y0 = 0; }
     };
 
@@ -82,14 +92,14 @@ conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
                 const int mt = tile % p.num_m_tiles;
                 const int n0 = (tile / p.num_m_tiles) * BN;
-                int b0, y0;
-                tile_origin(mt, b0, y0);
+                int b0, y0, x0;
+                tile_origin(mt, b0, y0, x0);
                 for (int kb = 0; kb < num_k_blocks; ++kb) {
                     const int tap = kb / p.kc_blocks, kc = kb - tap * p.kc_blocks;
                     int ax, ay, wtap;
                     if (MODE == 1) {
                         const int ky = tap >> 2, kx = tap & 3;
-                        ax = kx - 1;                     // 2*0 - 1 + kx (tiles span the full output width)
+                        ax = 2 * x0 - 1 + kx;
                         ay = 2 * y0 - 1 + ky;
                         wtap = tap;
                     } else {
@@ -99,7 +109,7 @@ conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
                         const int kx = p.px == 0 ? (tx == 0 ? 1 : 3) : (tx == 0 ? 0 : 2);
                         const int dy = p.py == 0 ? (ty == 0 ? 0 : -1) : (ty == 0 ? 1 : 0);
                         const int dx = p.px == 0 ? (tx == 0 ? 0 : -1) : (tx == 0 ? 1 : 0);
-                        ax = dx;
+                        ax = x0 + dx;
                         ay = y0 + dy;
                         wtap = ky * 4 + kx;
                     }
@@ -145,17 +155,18 @@ conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             wgmma_wait<0>();
             fence_regs(acc);
             if (lane == 0) mbar_arrive(&empty_bar[prev]);
-            int b0, y0;
-            tile_origin(mt, b0, y0);
+            int b0, y0, x0;
+            tile_origin(mt, b0, y0, x0);
             size_t out_row[2];
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int r = r_in + 8 * h;
-                if (MODE == 1) {
+                if (MODE == 1) {   // tiles are consecutive 128-pixel runs of the NHWC output in every tiling
                     out_row[h] = (size_t)mt * BM + r;
                 } else {   // tile row r = x + W * j, j = (image - b0) * TH + (row - y0) on the input grid
+                           // (row segments: j = 0, x = r, input column x0 + r)
                     const int j = r / p.W, x = r % p.W;
-                    out_row[h] = ((size_t)2 * (b0 * p.H + y0 + j) + p.py) * (2 * p.W) + 2 * x + p.px;
+                    out_row[h] = ((size_t)2 * (b0 * p.H + y0 + j) + p.py) * (2 * p.W) + 2 * (x0 + x) + p.px;
                 }
             }
 #pragma unroll
@@ -193,7 +204,14 @@ int launch_conv(const CUtensorMap& tmA, const CUtensorMap& tmB, const ConvParams
 
 // fills the tile decomposition for a [B, H, W] pixel grid; returns false if it cannot be tiled by 128
 bool plan_tiles(int B, int H, int W, ConvParams& p) {
-    if (!pow2(W) || !pow2(H) || W > 128) return false;
+    if (W > BM) {   // row segments
+        if (W % BM != 0 || H < 1) return false;
+        p.H = H; p.W = W;
+        p.NB = 1; p.TH = 1; p.row_segs = W / BM; p.tiles_per_image = H * p.row_segs;
+        p.num_m_tiles = B * p.tiles_per_image;
+        return true;
+    }
+    if (!pow2(W) || !pow2(H)) return false;
     p.H = H; p.W = W;
     if (H * W >= 128) {
         p.NB = 1; p.TH = 128 / W; p.tiles_per_image = (H * W) / 128;
@@ -215,7 +233,8 @@ extern "C" int cv_conv2d_k4s2(const void* x, const void* w_packed, const void* b
     CV_REQUIRE(IH % 2 == 0 && IW % 2 == 0, "input height/width must be even");
     const int OH = IH / 2, OW = IW / 2;
     ConvParams p = {};
-    CV_REQUIRE(plan_tiles(B, OH, OW, p), "output H, W must be powers of two, W <= 128, and 128 pixels must tile the batch");
+    CV_REQUIRE(plan_tiles(B, OH, OW, p), "output W must be a power of two <= 128 (with H a power of two and 128 pixels "
+                                         "tiling the batch) or a multiple of 128");
     p.Cin = Cin; p.Cout = Cout; p.kc_blocks = Cin / 64; p.ntaps = 16; p.bias = static_cast<const __nv_bfloat16*>(bias);
     p.relu = relu;
     const int BN = (Cout % 256 == 0) ? 256 : 128;
@@ -225,9 +244,15 @@ extern "C" int cv_conv2d_k4s2(const void* x, const void* w_packed, const void* b
     {   // input NHWC as [C, W, H, B], traversal stride 2 in W and H
         uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)IW, (uint64_t)IH, (uint64_t)B};
         uint64_t str[3] = {(uint64_t)Cin * 2, (uint64_t)IW * Cin * 2, (uint64_t)IH * IW * Cin * 2};
-        uint32_t box[4] = {64, (uint32_t)(2 * OW), (uint32_t)(2 * p.TH), (uint32_t)p.NB};
         uint32_t es[4] = {1, 2, 2, 1};
-        int rc = cvh::encode_tmap(&tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, x, dims, str, box, es, cvh::Swizzle::B128);
+        int rc;
+        if (p.row_segs > 0) {   // 128 output columns of one output row
+            uint32_t box[4] = {64, (uint32_t)(2 * BM), 2, 1};
+            rc = cvh::encode_tmap(&tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, x, dims, str, box, es, cvh::Swizzle::B128);
+        } else {
+            uint32_t box[4] = {64, (uint32_t)(2 * OW), (uint32_t)(2 * p.TH), (uint32_t)p.NB};
+            rc = cvh::encode_tmap(&tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, x, dims, str, box, es, cvh::Swizzle::B128);
+        }
         if (rc) return rc;
     }
     int rc = cvh::encode_tmap_2d_bf16(&tmB, w_packed, (uint64_t)16 * Cout, Cin, Cin, BN, 64);
@@ -241,7 +266,8 @@ extern "C" int cv_conv_transpose2d_k4s2(const void* x, const void* w_packed, con
     CV_REQUIRE(x && w_packed && y, "null pointer");
     CV_REQUIRE(Cin % 64 == 0 && Cout % 128 == 0, "Cin must be a multiple of 64 and Cout of 128");
     ConvParams p = {};
-    CV_REQUIRE(plan_tiles(B, IH, IW, p), "input H, W must be powers of two, W <= 128, and 128 pixels must tile the batch");
+    CV_REQUIRE(plan_tiles(B, IH, IW, p), "input W must be a power of two <= 128 (with H a power of two and 128 pixels "
+                                         "tiling the batch) or a multiple of 128");
     p.Cin = Cin; p.Cout = Cout; p.kc_blocks = Cin / 64; p.ntaps = 4; p.bias = static_cast<const __nv_bfloat16*>(bias);
     p.relu = relu;
     const int BN = (Cout % 256 == 0) ? 256 : 128;
@@ -251,9 +277,16 @@ extern "C" int cv_conv_transpose2d_k4s2(const void* x, const void* w_packed, con
     {   // input NHWC as [C, W, H, B], unit strides; halo taps fall outside and are zero-filled
         uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)IW, (uint64_t)IH, (uint64_t)B};
         uint64_t str[3] = {(uint64_t)Cin * 2, (uint64_t)IW * Cin * 2, (uint64_t)IH * IW * Cin * 2};
-        uint32_t box[4] = {64, (uint32_t)IW, (uint32_t)p.TH, (uint32_t)p.NB};
-        int rc = cvh::encode_tmap(&tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, x, dims, str, box, nullptr,
+        int rc;
+        if (p.row_segs > 0) {   // 128 input columns of one input row
+            uint32_t box[4] = {64, (uint32_t)BM, 1, 1};
+            rc = cvh::encode_tmap(&tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, x, dims, str, box, nullptr,
                                   cvh::Swizzle::B128);
+        } else {
+            uint32_t box[4] = {64, (uint32_t)IW, (uint32_t)p.TH, (uint32_t)p.NB};
+            rc = cvh::encode_tmap(&tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, x, dims, str, box, nullptr,
+                                  cvh::Swizzle::B128);
+        }
         if (rc) return rc;
     }
     int rc = cvh::encode_tmap_2d_bf16(&tmB, w_packed, (uint64_t)16 * Cout, Cin, Cin, BN, 64);

@@ -5,6 +5,7 @@ through the VQ-VAE.  Text <-> string conversion (sentencepiece) and image file I
 import torch
 
 from . import vqvae
+from .generation.magnify import magnify
 from .generation.sampling import add_interlacing_beam_marks, filling_sequence, get_tokenizer
 
 # generate_samples.py:203-214
@@ -103,3 +104,22 @@ def generate_images_once(model, vq_model, args, seq, num=8, fill=filling_sequenc
                 img = torch.nn.functional.interpolate(img, size=(256, 256))
             imgs.append(img)
     return rows, torch.cat(imgs, dim=0)
+
+
+def super_resolution(model, vq_model, args, seq, fill=filling_sequence, decode=None, debug=False):
+    """generate_samples.py:223-244: `seq` is the 'super-resolution' template filled in, [ROI1] text [BASE] [BOI1]
+    followed by the 1024 codes of a 32 x 32 source image.  The source is magnified to 64 x 64 codes by `magnify`'s
+    nine windows, and the grid is decoded by the VQ-VAE.  Returns (codes [1, 4096], images [n, 3, 512, 512]); n = 1,
+    or 2 with debug=True, when the source image decoded and interpolated to 512 x 512 comes first, as the
+    reference's debug output does."""
+    decode = decode or (lambda codes: vqvae.code2img(vq_model, codes))
+    tok = get_tokenizer(args)
+    model.eval()
+    with torch.no_grad():
+        codes = magnify(model, tok, seq[-1024:], seq[:-1024], args, fill=fill)
+        imgs = []
+        if debug:
+            src = decode(seq[-1024:].view(1, 32, 32))
+            imgs.append(torch.nn.functional.interpolate(src, size=(512, 512)))
+        imgs.append(decode(codes.view(1, 64, 64)))
+    return codes, torch.cat(imgs, dim=0)

@@ -142,7 +142,9 @@ class Decoder(nn.Module):
             nn.ConvTranspose2d(channel, channel, 4, stride=2, padding=1), nn.ReLU(inplace=True),
             nn.Conv2d(channel, out_channel, 1))
         self._cache = _PackCache()
-        self.batch_chunk = 16                   # images per pass: the last activation is 67 MB / image in bf16
+        # images per pass at 256 x 256 output, where the last activation is 67 MB / image in bf16; larger outputs
+        # take proportionally fewer images per pass (4 at 512 x 512)
+        self.batch_chunk = 16
 
     def _packed(self):
         b = self.blocks
@@ -161,9 +163,11 @@ class Decoder(nn.Module):
         dev = quant_nhwc.device
         one = torch.ones(3, device=dev) if scale is None else scale
         zero = torch.zeros(3, device=dev) if shift is None else shift
+        h, w = quant_nhwc.shape[1], quant_nhwc.shape[2]
+        chunk = max(1, min(self.batch_chunk, self.batch_chunk * 256 * 256 // (8 * h * 8 * w)))
         outs = []
-        for b0 in range(0, quant_nhwc.shape[0], self.batch_chunk):
-            x = quant_nhwc[b0:b0 + self.batch_chunk].contiguous()
+        for b0 in range(0, quant_nhwc.shape[0], chunk):
+            x = quant_nhwc[b0:b0 + chunk].contiguous()
             x = ops.conv_transpose2d_k4s2(x, P['w0'], P['b0'], relu=True)
             x = ops.conv_transpose2d_k4s2(x, P['w2'], P['b2'], relu=True)
             x = ops.conv_transpose2d_k4s2(x, P['w4'], P['b4'], relu=True)

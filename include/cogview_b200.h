@@ -337,8 +337,10 @@ int cv_clip_coef(const float* sumsq, float max_norm, float* coef, float* norm_ou
  *     Encoder (vqvae_zc.py:121-129) and Decoder (:172-191) as im2col-free implicit GEMMs on wgmma: A tiles are
  *     TMA boxes of the NHWC input (traversal stride 2 / sub-pixel phases, zero-filled halo = padding).
  *     x: [B, IH, IW, Cin]; w_packed: [16 (ky*4+kx), Cout, Cin] bf16; bias bf16 [Cout] or NULL; relu fused.
- *     y: [B, IH/2, IW/2, Cout] (conv) or [B, 2IH, 2IW, Cout] (transposed).  Cin % 64 == 0, Cout % 128 == 0,
- *     tile-grid H, W powers of two with W <= 128.
+ *     y: [B, IH/2, IW/2, Cout] (conv) or [B, 2IH, 2IW, Cout] (transposed).  Cin % 64 == 0, Cout % 128 == 0.
+ *     Tile grid (output for the conv, input for the transposed conv) [B, H, W]: either H, W powers of two with
+ *     W <= 128 (128-pixel tiles of whole rows or whole images; B must be a multiple of 128 / (H W) when H W < 128),
+ *     or W > 128 with W % 128 == 0 and any H >= 1 (128-pixel row segments).  Other shapes are refused.
  *   cv_im2col_k4s2_c3: patches of the fp32 NCHW 3-channel image -> [B*OH*OW, 64] bf16 (48 used) for the first conv
  *     (run as cv_gemm_bf16 with act = 2).
  *   cv_vq_split3 / cv_vq_argmin / cv_vq_lookup: Quantize.forward_ hard path (vqvae_zc.py:41-54) and embed_code (:95-96);
