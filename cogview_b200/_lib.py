@@ -52,6 +52,8 @@ def _declare(lib):
         "cv_attn_bwd": [P, L, L, P, L, L, P, L, L, P, P, P, P, P, I, I, I, I, I, F, P, P],
         "cv_linear_small_m": [P, L, P, L, P, P, L, I, I, P, I, I, I, P],
         "cv_ln_pair_small_m": [P, P, P, P, P, P, P, F, P, P, I, I, P],
+        "cv_linear_mid_m": [P, L, P, L, P, P, L, I, I, P, I, I, I, P],
+        "cv_ln_pair_mid_m": [P, P, P, P, P, P, P, F, P, P, I, I, P],
         "cv_attn_gather": [P, L, L, P, L, P, P, I, I, I, I, I, P],
         "cv_attn_decode": [P, P, L, P, I, P, P, I, I, I, I, I, P],
         "cv_sparse_plan": [P, L, P, I, I, I, I, I, P, P, I, P, P, P],

@@ -6,7 +6,7 @@ import torch
 
 from . import vqvae
 from .generation.magnify import magnify
-from .generation.sampling import add_interlacing_beam_marks, filling_sequence, get_tokenizer
+from .generation.sampling import add_interlacing_beam_marks, filling_sequence, get_tokenizer, inverse_prompt_score
 
 # generate_samples.py:203-214
 QUERY_TEMPLATES = {
@@ -123,3 +123,26 @@ def super_resolution(model, vq_model, args, seq, fill=filling_sequence, decode=N
             imgs.append(torch.nn.functional.interpolate(src, size=(512, 512)))
         imgs.append(decode(codes.view(1, 64, 64)))
     return codes, torch.cat(imgs, dim=0)
+
+
+def post_selection_rows(rows, text, tokenizer=None):
+    """The 'post-selection' query of every row `generate_images_once` returned: [BASE] [BOI1] codes [EOI1] [ROI1] text,
+    where codes is the row's last image (the generated one) and `text` the caption's token ids (already offset into the
+    unified vocabulary).  Returns a LongTensor [num, 2 + 1024 + 2 + len(text)] on the rows' device."""
+    out = []
+    for row in rows:
+        _, images = split_tokens(row.tolist(), tokenizer)
+        out.append(build_query(QUERY_TEMPLATES['post-selection'], [images[-1], text], tokenizer))
+    return torch.tensor(out, dtype=torch.long, device=rows.device)
+
+
+def post_selection(model, args, seq, score=inverse_prompt_score):
+    """generate_samples.py:246-270 without the file output: `seq` holds one post-selection query per row ([num, len],
+    see post_selection_rows); returns the caption log-likelihood of every row, scores [num], computed in groups of
+    args.max_inference_batch_size rows.  The best candidates are scores.topk(k).indices."""
+    num = seq.shape[0]
+    mbz = args.max_inference_batch_size
+    assert num < mbz or num % mbz == 0
+    model.eval()
+    with torch.no_grad():
+        return torch.cat([score(model, seq[i * mbz:(i + 1) * mbz], args) for i in range(max(num // mbz, 1))], dim=0)

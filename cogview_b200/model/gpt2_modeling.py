@@ -117,7 +117,8 @@ def _fast_decode_impl(self, input_ids, position_ids, mems, b, sq):
     replay of the weight-streaming decode step.  Returns None when the call does not qualify."""
     tr = self.transformer
     if (sq != 1 or not mems or tr.mems_mode != 'kv' or tr.max_memory_length <= 0 or torch.is_grad_enabled()
-            or b > 16 or os.environ.get('COGVIEW_B200_FAST_DECODE', '1') == '0'):
+            or not ops.decode_batch_supported(b, tr.hidden_size)
+            or os.environ.get('COGVIEW_B200_FAST_DECODE', '1') == '0'):
         return None
     from ..mpu import kv_cache
     from ..mpu.decode import DecodeRunner
@@ -143,8 +144,9 @@ def _generate_run_impl(self, last_tokens, first_pos, mems, n_steps, temperature,
     token, chosen on the device (cv_sparse_plan) instead of Python's random.sample — same distribution, other stream."""
     tr = self.transformer
     b = last_tokens.shape[0]
-    if (not mems or tr.mems_mode != 'kv' or tr.max_memory_length <= 0 or torch.is_grad_enabled() or b > 16
-            or n_steps < 1 or os.environ.get('COGVIEW_B200_FAST_DECODE', '1') == '0'
+    if (not mems or tr.mems_mode != 'kv' or tr.max_memory_length <= 0 or torch.is_grad_enabled()
+            or not ops.decode_batch_supported(b, tr.hidden_size) or n_steps < 1
+            or os.environ.get('COGVIEW_B200_FAST_DECODE', '1') == '0'
             or os.environ.get('COGVIEW_B200_GRAPH_SAMPLING', '1') == '0'):
         return None
     from ..mpu import kv_cache
@@ -157,7 +159,8 @@ def _generate_run_impl(self, last_tokens, first_pos, mems, n_steps, temperature,
         runner = caches.runner = DecodeRunner(self, caches,
                                               use_graph=os.environ.get('COGVIEW_B200_CUDA_GRAPH', '1') != '0')
     pos = torch.full((b, 1), int(first_pos), dtype=torch.long, device=last_tokens.device)
-    if sparse is not None and (b > 16 or tr.max_memory_length > 4096 or runner.persistent):
+    # sparse inference: cv_sparse_plan is written for at most 16 sequences
+    if sparse is not None and (b > ops.DECODE_SMALL_MAX_BATCH or tr.max_memory_length > 4096 or runner.persistent):
         return None
     new_tokens, logp = runner.sample_run(last_tokens.reshape(b, 1), pos, caches.t, n_steps, temperature, top_k,
                                          invalid_slices, sparse=sparse)

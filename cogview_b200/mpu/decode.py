@@ -4,8 +4,9 @@ This is the fast path behind GPT2Model.forward when it is called the way generat
 it (one new token per sequence, `mems` returned by the previous call, mems_mode 'kv').
 
 Two device paths:
-  * default: one kernel per operation (cv_linear_small_m, cv_attn_decode, cv_ln_pair_small_m; batch <= 16), CUDA-graph
-    captured; in generation runs followed by ONE sampling kernel (cv_sample_topk) inside the same graph.
+  * default: one kernel per operation (cv_attn_decode between cv_linear_small_m / cv_ln_pair_small_m at batch <= 16,
+    cv_linear_mid_m / cv_ln_pair_mid_m at batch 17..64), CUDA-graph captured; in generation runs followed by ONE
+    sampling kernel (cv_sample_topk) inside the same graph.
   * COGVIEW_B200_PERSISTENT=1 and batch <= 8: the whole step — embedding, 48 Sandwich-LN layers, final LayerNorm,
     logits — is ONE persistent kernel (cv_decode_step, csrc/decode_step.cu: bulk-copy weight stream through a
     shared-memory byte ring, register-resident residual stream, grid barriers between the dependency points).  Parity-
@@ -39,6 +40,11 @@ class DecodeRunner:
         self.step_logits = None          # output buffer of the step (static: graphs write into it)
         self.graph = None
         self.use_graph = use_graph
+        assert self.b <= ops.DECODE_MAX_BATCH
+        # which pair of kernels runs the linears and the Sandwich-LN glue is a property of the batch size
+        small = self.b <= ops.DECODE_SMALL_MAX_BATCH
+        self.linear = ops.linear_small_m if small else ops.linear_mid_m
+        self.ln_pair = ops.ln_pair_small_m if small else ops.ln_pair_mid_m
         self.persistent = (_persistent_enabled() and self.b <= ops.DECODE_STEP_MAX_BATCH and self.h % 256 == 0
                            and self.h <= 2560)
         # enough (batch, head, split) CTAs to cover the SMs
@@ -131,27 +137,27 @@ class DecodeRunner:
             (g1, b1, wqkv, bqkv, wd, bd, g3, b3, g2, b2, w1, bb1, w2, bb2, g4, b4) = P
             s = scal[2 * i:2 * i + 2]
             # x_i = x_{i-1} + LN4(mlp_out_{i-1});  xn = LN1(x_i)
-            y, xn = ops.ln_pair_small_m(x, prev_gemm, prev_am, prev_post, (g1, b1), self.eps,
-                                        want_res_out=prev_gemm is not None)
+            y, xn = self.ln_pair(x, prev_gemm, prev_am, prev_post, (g1, b1), self.eps,
+                                 want_res_out=prev_gemm is not None)
             if y is not None:
                 x = y
-            qkv = ops.linear_small_m(xn, wqkv, bqkv)
+            qkv = self.linear(xn, wqkv, bqkv)
             if sparse is not None:
                 ctx = ops.attn_decode_gather(qkv, self.caches.buf[i], heads, self.cur_len, self.key_idx[i], self.n_keys,
                                              nsplit=self.nsplit)
             else:
                 ctx = ops.attn_decode(qkv, self.caches.buf[i], heads, cur_len_dev=self.cur_len, nsplit=self.nsplit)
-            attn_out = ops.linear_small_m(ctx, wd, bd, absmax=s[0:1])
+            attn_out = self.linear(ctx, wd, bd, absmax=s[0:1])
             # y = x + LN3(attn_out);  xn2 = LN2(y)
-            x, xn2 = ops.ln_pair_small_m(x, attn_out, s[0:1], (g3, b3), (g2, b2), self.eps)
-            h4 = ops.linear_small_m(xn2, w1, bb1, act=ops.ACT_GELU)
-            prev_gemm = ops.linear_small_m(h4, w2, bb2, absmax=s[1:2])
+            x, xn2 = self.ln_pair(x, attn_out, s[0:1], (g3, b3), (g2, b2), self.eps)
+            h4 = self.linear(xn2, w1, bb1, act=ops.ACT_GELU)
+            prev_gemm = self.linear(h4, w2, bb2, absmax=s[1:2])
             prev_am, prev_post = s[1:2], (g4, b4)
-        _, xf = ops.ln_pair_small_m(x, prev_gemm, prev_am, prev_post, (self.fl[0], self.fl[1]), self.fl[2],
-                                    want_res_out=False)
+        _, xf = self.ln_pair(x, prev_gemm, prev_am, prev_post, (self.fl[0], self.fl[1]), self.fl[2],
+                             want_res_out=False)
         if self.step_logits is None:
             self.step_logits = torch.empty((b, self.wte.shape[0]), dtype=torch.float32, device=self.ids.device)
-        return ops.linear_small_m(xf, self.wte, out=self.step_logits)
+        return self.linear(xf, self.wte, out=self.step_logits)
 
     def step(self, ids, pos, t):
         """ids, pos: [b, 1] int64; t: tokens already cached.  Returns logits [b, V] fp32 (a static buffer that the

@@ -59,14 +59,42 @@ class _Caches:
         return out
 
 
+# Caches of several batch sizes are kept so that a run that alternates between them (one prompt, then its beams)
+# does not re-allocate and re-capture; but at the 4B shape a 32-sequence and a 64-sequence cache together are 51 GB.
+# When the pooled caches would exceed this many bytes, those of the other batch sizes are dropped first.
+POOL_BYTE_BUDGET = 40 << 30
+
+
+def cache_bytes(owner, b):
+    return len(owner.layers) * b * owner.max_memory_length * 2 * owner.hidden_size * 2
+
+
+def _make_room(owner, pool, b):
+    """Called before a cache for batch size b is allocated: drop pooled caches of other sizes, largest first, until
+    the pool with the new cache fits POOL_BYTE_BUDGET (the new cache itself is always allowed)."""
+    need = cache_bytes(owner, b)
+    others = sorted((k for k in pool if k != b), key=lambda k: pool[k].buf.numel(), reverse=True)
+    total = need + sum(pool[k].buf.numel() * 2 for k in others)
+    for k in others:
+        if total <= POOL_BYTE_BUDGET:
+            break
+        total -= pool[k].buf.numel() * 2
+        if getattr(owner, '_kv', None) is pool[k]:
+            owner._kv = None
+        del pool[k]
+
+
 def prepare(owner, mems, b, sq):
     """Find (or build) the cache that `mems` refers to and get it ready for sq more tokens.  One cache (and its
-    captured decode graph) is kept per batch size and reused across sequences."""
+    captured decode graph) is kept per batch size and reused across sequences, within POOL_BYTE_BUDGET."""
     dev = owner.position_embeddings.weight.device
     pool = owner.__dict__.setdefault('_kv_pool', {})
     c = pool.get(b)
     if c is not None and (c.maxlen != owner.max_memory_length or c.buf.device != dev):
         c = None
+        del pool[b]
+    if c is None:
+        _make_room(owner, pool, b)
     if not mems:
         if c is None:
             c = _Caches(owner, b, dev)

@@ -303,18 +303,27 @@ def colsum(dy):
 # ----------------------------------------------------------------------------------------------------
 # decode (weight-streaming) kernels
 # ----------------------------------------------------------------------------------------------------
-def linear_small_m(x, w, bias=None, *, act=ACT_NONE, out_dtype=torch.bfloat16, absmax=None, out=None):
-    """y = x @ w^T + bias for 1 <= M <= 16 rows (x: [M,K] bf16, w: [N,K] bf16)."""
+def _decode_linear(name, x, w, bias, act, out_dtype, absmax, out):
     require_cuda(x, w, bias, absmax)
     M, K = x.shape
     N = w.shape[0]
     assert x.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and x.stride(1) == 1 and w.stride(1) == 1
     if out is None:
         out = torch.empty((M, N), dtype=out_dtype, device=x.device)
-    rc = lib().cv_linear_small_m(ptr(x), x.stride(0), ptr(w), w.stride(0), ptr(bias), ptr(out), out.stride(0),
-                                 int(out.dtype == torch.float32), int(act), ptr(absmax), M, N, K, stream_ptr())
-    check(rc, "cv_linear_small_m")
+    rc = getattr(lib(), name)(ptr(x), x.stride(0), ptr(w), w.stride(0), ptr(bias), ptr(out), out.stride(0),
+                              int(out.dtype == torch.float32), int(act), ptr(absmax), M, N, K, stream_ptr())
+    check(rc, name)
     return out
+
+
+def linear_small_m(x, w, bias=None, *, act=ACT_NONE, out_dtype=torch.bfloat16, absmax=None, out=None):
+    """y = x @ w^T + bias for 1 <= M <= 16 rows (x: [M,K] bf16, w: [N,K] bf16)."""
+    return _decode_linear("cv_linear_small_m", x, w, bias, act, out_dtype, absmax, out)
+
+
+def linear_mid_m(x, w, bias=None, *, act=ACT_NONE, out_dtype=torch.bfloat16, absmax=None, out=None):
+    """y = x @ w^T + bias for 17 <= M <= 64 rows (x: [M,K] bf16, w: [N,K] bf16)."""
+    return _decode_linear("cv_linear_mid_m", x, w, bias, act, out_dtype, absmax, out)
 
 
 def attn_decode(qkv, cache, heads, *, cur_len=None, cur_len_dev=None, nsplit=1, out=None, workspace=None):
@@ -368,21 +377,39 @@ def attn_decode_gather(qkv, cache, heads, cur_len_dev, idx, n_dev, *, nsplit=1, 
     return out
 
 
-def ln_pair_small_m(res_in, gemm_out, absmax_gemm, post, pre, eps, *, want_res_out=True):
-    """y = res_in + LN_post(gemm_out) (gemm_out may be None), xn = LN_pre(y).  post/pre: (gamma, beta) bf16.
-    Returns (y fp32 or None, xn bf16)."""
+def _decode_ln_pair(name, res_in, gemm_out, absmax_gemm, post, pre, eps, want_res_out):
     require_cuda(res_in, gemm_out)
     M, K = res_in.shape
     assert res_in.dtype == torch.float32 and res_in.is_contiguous()
     y = torch.empty_like(res_in) if want_res_out else None
     xn = torch.empty((M, K), dtype=torch.bfloat16, device=res_in.device)
     gp, bp = post if post is not None else (None, None)
-    rc = lib().cv_ln_pair_small_m(ptr(res_in), ptr(gemm_out), ptr(absmax_gemm), ptr(gp), ptr(bp), ptr(pre[0]),
-                                  ptr(pre[1]), float(eps), ptr(y), ptr(xn), M, K, stream_ptr())
-    check(rc, "cv_ln_pair_small_m")
+    rc = getattr(lib(), name)(ptr(res_in), ptr(gemm_out), ptr(absmax_gemm), ptr(gp), ptr(bp), ptr(pre[0]),
+                              ptr(pre[1]), float(eps), ptr(y), ptr(xn), M, K, stream_ptr())
+    check(rc, name)
     return y, xn
 
 
+def ln_pair_small_m(res_in, gemm_out, absmax_gemm, post, pre, eps, *, want_res_out=True):
+    """y = res_in + LN_post(gemm_out) (gemm_out may be None), xn = LN_pre(y).  post/pre: (gamma, beta) bf16.
+    1 <= M <= 16 rows.  Returns (y fp32 or None, xn bf16)."""
+    return _decode_ln_pair("cv_ln_pair_small_m", res_in, gemm_out, absmax_gemm, post, pre, eps, want_res_out)
+
+
+def ln_pair_mid_m(res_in, gemm_out, absmax_gemm, post, pre, eps, *, want_res_out=True):
+    """ln_pair_small_m for 17 <= M <= 64 rows."""
+    return _decode_ln_pair("cv_ln_pair_mid_m", res_in, gemm_out, absmax_gemm, post, pre, eps, want_res_out)
+
+
+# sequences per decode step: up to DECODE_SMALL_MAX_BATCH the *_small_m kernels, up to DECODE_MAX_BATCH the *_mid_m ones
+DECODE_SMALL_MAX_BATCH = 16
+DECODE_MAX_BATCH = 64
+LN_PAIR_MID_MAX_HIDDEN = 2560      # cv_ln_pair_mid_m keeps a row in the registers of 128 threads
+
+
+def decode_batch_supported(b, hidden):
+    """True if the per-operation decode kernels cover b sequences per step at this hidden size."""
+    return b <= DECODE_SMALL_MAX_BATCH or (b <= DECODE_MAX_BATCH and hidden <= LN_PAIR_MID_MAX_HIDDEN)
 DECODE_STEP_MAX_BATCH = 8
 
 

@@ -212,6 +212,17 @@ int cv_linear_small_m(const void* x, int64_t ldx, const void* W, int64_t ldw, co
 int cv_ln_pair_small_m(const float* res_in, const void* gemm_out, const float* absmax_gemm, const void* g_post,
                        const void* b_post, const void* g_pre, const void* b_pre, float eps, float* res_out,
                        void* xn_out, int M, int K, void* stream);
+/* The same two operations for 17 <= M <= 64 rows (csrc/decode_mid.cu), same arguments.
+ *   cv_linear_mid_m: TMA + wgmma weight streaming with the weights as the 64-row operand; K is split over the CTAs
+ *     of a thread-block cluster and reduced in a fixed order through distributed shared memory, so equal inputs give
+ *     equal bits.  W is read through a tensor map: ldw * 2 bytes must be a multiple of 16 (ldw % 8 == 0).
+ *   cv_ln_pair_mid_m: one cluster of ceil(M / 8) CTAs; max|y| over all rows is exchanged through distributed shared
+ *     memory.  K <= 2560. */
+int cv_linear_mid_m(const void* x, int64_t ldx, const void* W, int64_t ldw, const void* bias, void* out, int64_t ldo,
+                    int out_is_f32, int act, float* absmax, int M, int N, int K, void* stream);
+int cv_ln_pair_mid_m(const float* res_in, const void* gemm_out, const float* absmax_gemm, const void* g_post,
+                     const void* b_post, const void* g_pre, const void* b_pre, float eps, float* res_out, void* xn_out,
+                     int M, int K, void* stream);
 /* sparse_attention_inference (mpu/sparse_transformer.py:727-750): dense softmax over the gathered keys
  * K[idx], V[idx] (idx = pivots U trailing window, [b, n] int64; its last sq entries are the queries' own positions,
  * which get the causal -10000 above the diagonal).  q: [b, sq, heads*64] view; cache [b, max_len, 2*heads*64] (K|V)
