@@ -56,6 +56,7 @@ def _declare(lib):
         "cv_ln_pair_mid_m": [P, P, P, P, P, P, P, F, P, P, I, I, P],
         "cv_attn_gather": [P, L, L, P, L, P, P, I, I, I, I, I, P],
         "cv_attn_decode": [P, P, L, P, I, P, P, I, I, I, I, I, P],
+        "cv_attn_decode_ragged": [P, P, L, P, I, P, P, P, I, I, I, I, I, P],
         "cv_sparse_plan": [P, L, P, I, I, I, I, I, P, P, I, P, P, P],
         "cv_attn_decode_gather": [P, P, L, P, P, L, P, P, P, I, I, I, I, I, P],
         "cv_adamw_step": [P, P, P, P, P, L, F, F, F, F, F, I, P, F, P],

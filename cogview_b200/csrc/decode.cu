@@ -8,6 +8,8 @@
 //   cv_attn_decode    : one query per sequence against the K|V cache, with the new token's K/V appended
 //                       in the same kernel (standard_attention, mpu/sparse_transformer.py:652-673, for sq = 1,
 //                       where every cached key is visible)
+//   cv_attn_decode_ragged : the same with a cache length per sequence (t_b = cur_len - row_pad[b]), so sequences of
+//                       captions of different lengths share one decode batch
 #include "common.cuh"
 #include "host.h"
 #include "../../include/cogview_b200.h"
@@ -342,10 +344,13 @@ struct DecodeParams {
     const int* idx;
     int64_t idx_bs;
     const int* n_dev;
+    // RAGGED: row b holds *cur_len_dev - row_pad[b] cached tokens (0 <= row_pad[b] <= *cur_len_dev)
+    const int* row_pad;
 };
 
 // 8 lanes cooperate on one key (8 dims each); a warp covers 4 keys per iteration.
-template <bool GATHER>
+// RAGGED: every row has its own t; the split-K ranges below follow from it, so a split may be empty for short rows.
+template <bool GATHER, bool RAGGED>
 __global__ void __launch_bounds__(DA_WARPS * 32)
 attn_decode_kernel(const DecodeParams p) {
     __shared__ float s_m[DA_WARPS * 4], s_l[DA_WARPS * 4];
@@ -356,7 +361,8 @@ attn_decode_kernel(const DecodeParams p) {
     const int h = p.heads * HD;
     pdl_launch_dependents();
     pdl_wait();
-    const int t = p.cur_len_dev ? *p.cur_len_dev : p.cur_len;   // cached tokens; the new token sits at index t
+    // cached tokens of this row; the new token sits at index t
+    const int t = (p.cur_len_dev ? *p.cur_len_dev : p.cur_len) - (RAGGED ? p.row_pad[batch] : 0);
     const __nv_bfloat16* qrow = p.qkv + (size_t)batch * 3 * h + head * HD + sub * 8;
     float q[8];
     bf16x8_to_float(*reinterpret_cast<const uint4*>(qrow), q);
@@ -635,9 +641,11 @@ extern "C" int64_t cv_attn_decode_workspace_bytes(int b, int heads, int nsplit) 
     return (int64_t)b * heads * nsplit * (HD + 2) * sizeof(float);
 }
 
-extern "C" int cv_attn_decode(const void* qkv, void* cache, int64_t cache_batch_stride, const int* cur_len_dev,
-                              int cur_len, void* out, float* workspace, int b, int heads, int head_dim, int max_len,
-                              int nsplit, void* stream) {
+namespace {
+// cv_attn_decode and cv_attn_decode_ragged (row_pad == nullptr: every row holds the same cur_len tokens)
+int attn_decode_launch(const void* qkv, void* cache, int64_t cache_batch_stride, const int* cur_len_dev, int cur_len,
+                       const int* row_pad, void* out, float* workspace, int b, int heads, int head_dim, int max_len,
+                       int nsplit, void* stream) {
     CV_REQUIRE(qkv && cache && out, "null pointer");
     CV_REQUIRE(head_dim == HD, "head_dim must be 64");
     CV_REQUIRE(b > 0 && heads > 0 && max_len > 0 && nsplit >= 1 && nsplit <= 64, "bad sizes");
@@ -655,8 +663,13 @@ extern "C" int cv_attn_decode(const void* qkv, void* cache, int64_t cache_batch_
     p.heads = heads; p.nsplit = nsplit; p.max_len = max_len;
     p.scale_log2 = (1.0f / sqrtf((float)head_dim)) * 1.4426950408889634f;
     p.idx = nullptr; p.idx_bs = 0; p.n_dev = nullptr;
+    p.row_pad = row_pad;
     dim3 grid(heads, b, nsplit);
-    CV_CUDA(cvh::launch_pdl(attn_decode_kernel<false>, grid, dim3(DA_WARPS * 32), 0, s, true, p));
+    if (row_pad != nullptr) {
+        CV_CUDA(cvh::launch_pdl(attn_decode_kernel<false, true>, grid, dim3(DA_WARPS * 32), 0, s, true, p));
+    } else {
+        CV_CUDA(cvh::launch_pdl(attn_decode_kernel<false, false>, grid, dim3(DA_WARPS * 32), 0, s, true, p));
+    }
     cvh::count_launches(1);
     if (nsplit > 1) {
         CV_CUDA(cvh::launch_pdl(attn_decode_combine_kernel, dim3(heads, b), dim3(HD), 0, s, true,
@@ -664,6 +677,22 @@ extern "C" int cv_attn_decode(const void* qkv, void* cache, int64_t cache_batch_
         cvh::count_launches(1);
     }
     return 0;
+}
+}  // namespace
+
+extern "C" int cv_attn_decode(const void* qkv, void* cache, int64_t cache_batch_stride, const int* cur_len_dev,
+                              int cur_len, void* out, float* workspace, int b, int heads, int head_dim, int max_len,
+                              int nsplit, void* stream) {
+    return attn_decode_launch(qkv, cache, cache_batch_stride, cur_len_dev, cur_len, nullptr, out, workspace, b, heads,
+                              head_dim, max_len, nsplit, stream);
+}
+
+extern "C" int cv_attn_decode_ragged(const void* qkv, void* cache, int64_t cache_batch_stride, const int* cur_len_dev,
+                                     int cur_len, const int* row_pad, void* out, float* workspace, int b, int heads,
+                                     int head_dim, int max_len, int nsplit, void* stream) {
+    CV_REQUIRE(row_pad != nullptr, "null pointer");
+    return attn_decode_launch(qkv, cache, cache_batch_stride, cur_len_dev, cur_len, row_pad, out, workspace, b, heads,
+                              head_dim, max_len, nsplit, stream);
 }
 
 extern "C" int cv_attn_gather(const void* q, int64_t ldq, int64_t bsq, const void* cache, int64_t cache_batch_stride,
@@ -796,8 +825,9 @@ extern "C" int cv_attn_decode_gather(const void* qkv, void* cache, int64_t cache
     p.heads = heads; p.nsplit = nsplit; p.max_len = max_len;
     p.scale_log2 = (1.0f / sqrtf((float)head_dim)) * 1.4426950408889634f;
     p.idx = idx; p.idx_bs = idx_batch_stride; p.n_dev = n_dev;
+    p.row_pad = nullptr;
     dim3 grid(heads, b, nsplit);
-    CV_CUDA(cvh::launch_pdl(attn_decode_kernel<true>, grid, dim3(DA_WARPS * 32), 0, s, true, p));
+    CV_CUDA(cvh::launch_pdl(attn_decode_kernel<true, false>, grid, dim3(DA_WARPS * 32), 0, s, true, p));
     cvh::count_launches(1);
     if (nsplit > 1) {
         CV_CUDA(cvh::launch_pdl(attn_decode_combine_kernel, dim3(heads, b), dim3(HD), 0, s, true,

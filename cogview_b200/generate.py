@@ -6,7 +6,8 @@ import torch
 
 from . import vqvae
 from .generation.magnify import magnify
-from .generation.sampling import add_interlacing_beam_marks, filling_sequence, get_tokenizer, inverse_prompt_score
+from .generation.sampling import (add_interlacing_beam_marks, filling_sequence, filling_sequences, get_tokenizer,
+                                  inverse_prompt_score)
 
 # generate_samples.py:203-214
 QUERY_TEMPLATES = {
@@ -95,15 +96,46 @@ def generate_images_once(model, vq_model, args, seq, num=8, fill=filling_sequenc
         for _ in range(max(num // mbz, 1)):
             rows.append(fill(model, seq.clone(), args))
         rows = torch.cat(rows, dim=0)
-        imgs = []
-        for row in rows:
-            _, images = split_tokens(row.tolist())
-            codes = torch.tensor(images[-1], dtype=torch.long, device=rows.device).unsqueeze(0)
-            img = decode(codes)
-            if img.shape[-1] == 128:                       # low-level super-resolution sources are 128 x 128
-                img = torch.nn.functional.interpolate(img, size=(256, 256))
-            imgs.append(img)
-    return rows, torch.cat(imgs, dim=0)
+        return rows, _decode_rows(rows, decode)
+
+
+def _decode_rows(rows, decode):
+    """The last image of every token row, decoded: [rows, 3, H, W]."""
+    imgs = []
+    for row in rows:
+        _, images = split_tokens(row.tolist())
+        codes = torch.tensor(images[-1], dtype=torch.long, device=rows.device).unsqueeze(0)
+        img = decode(codes)
+        if img.shape[-1] == 128:                       # low-level super-resolution sources are 128 x 128
+            img = torch.nn.functional.interpolate(img, size=(256, 256))
+        imgs.append(img)
+    return torch.cat(imgs, dim=0)
+
+
+def generate_images_batch(model, vq_model, args, seqs, num=8, fill=filling_sequences, decode=None):
+    """generate_images_once for a list of templates (e.g. one per caption of a caption file): returns one
+    (token rows [num, len(seq)], images [num, 3, H, W]) pair per template.  With num <= args.max_inference_batch_size
+    whole templates are packed into decode batches of at most that many rows (`fill` takes a list of templates and
+    returns a list of token tensors, see filling_sequences); above it every template runs through generate_images_once
+    on its own."""
+    decode = decode or (lambda codes: vqvae.code2img(vq_model, codes))
+    mbz = args.max_inference_batch_size
+    if num > mbz:
+        return [generate_images_once(model, vq_model, args, seq, num=num, fill=lambda m, s, a: fill(m, [s], a)[0],
+                                     decode=decode) for seq in seqs]
+    per_group = mbz // num
+    out = []
+    model.eval()
+    with torch.no_grad():
+        for g0 in range(0, len(seqs), per_group):
+            group = []
+            for seq in seqs[g0:g0 + per_group]:
+                seq = seq.clone()
+                add_interlacing_beam_marks(seq, nb=num)
+                group.append(seq)
+            for rows in fill(model, group, args):
+                out.append((rows, _decode_rows(rows, decode)))
+    return out
 
 
 def super_resolution(model, vq_model, args, seq, fill=filling_sequence, decode=None, debug=False):

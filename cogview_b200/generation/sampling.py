@@ -145,6 +145,41 @@ def add_interlacing_beam_marks(seq, nb=12, period=3000):
             blk_cnt = 0
 
 
+def _slices_after(tokenizer, tok, cur):
+    """The vocabulary slices that may not be sampled after token `tok` ([BOI*]: only image codes, [EOI*]: only text)."""
+    n_img = tokenizer.img_tokenizer.num_tokens
+    n_txt = tokenizer.txt_tokenizer.num_tokens
+    if tok in (tokenizer['[BOI1]'], tokenizer['[BOI2]']):
+        return [slice(n_img, None)]
+    if tok in (tokenizer['[EOI1]'], tokenizer['[EOI2]']):
+        return [slice(0, n_img), slice(n_img + n_txt, None)]
+    return cur
+
+
+def _scan_context(tmpl, tokenizer):
+    """(context length, position offset of the last [ROI2] in the context or 100000, invalid slices after the
+    context) of a template list."""
+    offset = 100000
+    invalid_slices = [slice(0, tokenizer.img_tokenizer.num_tokens)]
+    context_length = 0
+    while context_length < len(tmpl) and tmpl[context_length] >= 0:
+        invalid_slices = _slices_after(tokenizer, tmpl[context_length], invalid_slices)
+        if tmpl[context_length] == tokenizer['[ROI2]']:
+            offset = context_length
+        context_length += 1
+    return context_length, offset, invalid_slices
+
+
+def _next_token_probs(logits, invalid_slices, args):
+    """Sampling distribution [b, V] from the last position's logits [b, s, V] (modified in place)."""
+    logits = logits[:, -1]
+    logits /= args.temperature
+    for sl in invalid_slices:
+        logits[..., sl] = -float('Inf')
+    logits = top_k_logits(logits, top_k=args.top_k, top_p=args.top_p)
+    return F.softmax(logits, dim=-1)
+
+
 def filling_sequence(model, seq, args, mems=None, invalid_slices=[], **kwargs):
     """generation/sampling.py:64-186.  seq: 1-D LongTensor template [ctx..., -N (generate with N beams), ...].
     Returns the filled token rows [nb, len(seq)]."""
@@ -154,26 +189,12 @@ def filling_sequence(model, seq, args, mems=None, invalid_slices=[], **kwargs):
     tmpl = seq.tolist()
     out_seq_length = len(tmpl)
     n_img = tokenizer.img_tokenizer.num_tokens
-    n_txt = tokenizer.txt_tokenizer.num_tokens
-    boi = (tokenizer['[BOI1]'], tokenizer['[BOI2]'])
-    eoi = (tokenizer['[EOI1]'], tokenizer['[EOI2]'])
     roi2 = tokenizer['[ROI2]']
-    offset = 100000
-    invalid_slices = [slice(0, n_img)]
 
     def slices_after(tok, cur):
-        if tok in boi:
-            return [slice(n_img, None)]
-        if tok in eoi:
-            return [slice(0, n_img), slice(n_img + n_txt, None)]
-        return cur
+        return _slices_after(tokenizer, tok, cur)
 
-    context_length = 0
-    while context_length < out_seq_length and tmpl[context_length] >= 0:
-        invalid_slices = slices_after(tmpl[context_length], invalid_slices)
-        if tmpl[context_length] == roi2:
-            offset = context_length
-        context_length += 1
+    context_length, offset, invalid_slices = _scan_context(tmpl, tokenizer)
     tokens, attention_mask, position_ids = get_batch(seq[:context_length], device, args)
 
     counter = context_length - 1
@@ -245,12 +266,7 @@ def filling_sequence(model, seq, args, mems=None, invalid_slices=[], **kwargs):
         counter += 1
         index += 1
 
-        logits = logits[:, -1]
-        logits /= args.temperature
-        for sl in invalid_slices:
-            logits[..., sl] = -float('Inf')
-        logits = top_k_logits(logits, top_k=args.top_k, top_p=args.top_p)
-        log_probs = F.softmax(logits, dim=-1)
+        log_probs = _next_token_probs(logits, invalid_slices, args)
 
         if nb > 1 and tokens.shape[0] == 1:     # 1 -> nb beams
             tokens = tokens.expand(nb, -1).contiguous()
@@ -268,6 +284,80 @@ def filling_sequence(model, seq, args, mems=None, invalid_slices=[], **kwargs):
             img_indices_bool = tokens < n_img
             txt_indices_bool = ~img_indices_bool
     return tokens.view(tokens.shape[0], -1).contiguous()
+
+
+def _batch_plan(model, tmpls, args, tokenizer):
+    """Per template (context length, [ROI2] offset, beam count, generate slots), and whether filling_sequences can
+    run all of them as one decode batch: every template is a context followed by one run of at least three generate
+    slots of the same beam count, to its end; all share the slot count, the beam count and the invalid slices; dense
+    attention on the K|V cache without nucleus sampling; at most ops.DECODE_MAX_BATCH rows; and the graph-replayed
+    decode path is on."""
+    from .. import ops
+    plans, keys = [], set()
+    ok = (getattr(args, 'is_sparse', 0) == 0 and args.top_p == 0.0 and hasattr(model, 'generate_run')
+          and not torch.is_grad_enabled())
+    for tmpl in tmpls:
+        C, offset, inv = _scan_context(tmpl, tokenizer)
+        gen = tmpl[C:]
+        nb = -gen[0] if gen else 0
+        plans.append((C, offset, nb, len(gen)))
+        keys.add((nb, len(gen), tuple((sl.start, sl.stop) for sl in inv)))
+        run = len(gen) - 1              # the first slot is drawn from the prompt's own forward
+        ok = ok and C > 0 and nb > 0 and run >= 2 and all(x == -nb for x in gen) and not (C <= offset < C + run)
+    tr = getattr(model, 'transformer', None)
+    rows = sum(p[2] for p in plans)
+    ok = (ok and len(keys) == 1 and tr is not None and getattr(tr, 'mems_mode', None) == 'kv'
+          and rows <= ops.DECODE_MAX_BATCH and ops.decode_batch_supported(rows, tr.hidden_size)
+          and max(p[0] for p in plans) + plans[0][3] - 1 <= tr.max_memory_length
+          and _os.environ.get('COGVIEW_B200_FAST_DECODE', '1') != '0'
+          and _os.environ.get('COGVIEW_B200_GRAPH_SAMPLING', '1') != '0')
+    return plans, ok
+
+
+def filling_sequences(model, seqs, args):
+    """filling_sequence for several templates (1-D LongTensors, e.g. one per caption) at once: returns one token tensor
+    [nb, len(seq_c)] per template.  Each context is run through the model on its own (batch 1) and its nb first tokens
+    are drawn as filling_sequence draws them; then the generate slots of all rows run as ONE decode batch (DecodeRunner
+    in ragged mode: every row continues at its own context length and position).  Templates that cannot share a batch
+    (see _batch_plan) are filled one by one with filling_sequence, as is a single template.
+    The abs-max LayerNorm scales of the decode step are taken over the whole batch, so a template's rows match a run
+    of that template alone within bf16 tolerance, not bit for bit."""
+    if len(seqs) == 1:
+        return [filling_sequence(model, seqs[0], args)]
+    tokenizer = get_tokenizer(args)
+    tmpls = [seq.tolist() for seq in seqs]
+    plans, ok = _batch_plan(model, tmpls, args, tokenizer)
+    if not ok:
+        return [filling_sequence(model, seq, args) for seq in seqs]
+    from ..mpu import kv_cache
+    device = seqs[0].device
+    prefixes, caption_mems, first_pos = [], [], []
+    for seq, tmpl, (C, offset, nb, n_gen) in zip(seqs, tmpls, plans):
+        _, _, invalid_slices = _scan_context(tmpl, tokenizer)
+        tokens, attention_mask, position_ids = get_batch(seq[:C], device, args)
+        position_ids = position_ids.clone()
+        position_ids[position_ids > offset] -= offset
+        logits, *mems = model(tokens, position_ids, attention_mask, None, None, 0)
+        # the batch-1 cache is reused by the next prompt's forward: keep a copy of this prompt's K|V
+        caption_mems.append([m.clone() for m in mems])
+        probs = _next_token_probs(logits, invalid_slices, args)
+        prev = torch.multinomial(probs, num_samples=nb, replacement=True) if nb > 1 else torch.multinomial(probs, 1)
+        prefixes.append(torch.cat((tokens.expand(nb, -1), prev.view(nb, 1)), dim=1))
+        first_pos += [C - offset if C > offset else C] * nb
+    run = plans[0][3] - 1
+    mems, row_pad = kv_cache.assemble(model.transformer, caption_mems, [p[2] for p in plans], run)
+    last = torch.cat([p[:, -1:] for p in prefixes], dim=0)
+    res = model.generate_run(last, first_pos, mems, run, args.temperature, args.top_k, invalid_slices,
+                             row_pad=row_pad)
+    if res is None:
+        raise RuntimeError('filling_sequences: the decode batch of %d rows was refused' % last.shape[0])
+    new_tokens = res[0]
+    out, r0 = [], 0
+    for p in prefixes:
+        nb = p.shape[0]
+        out.append(torch.cat((p, new_tokens[r0:r0 + nb].to(p.device)), dim=1))
+        r0 += nb
+    return out
 
 
 def inverse_prompt_score(model, seq, args):

@@ -134,14 +134,18 @@ def _fast_decode_impl(self, input_ids, position_ids, mems, b, sq):
 GPT2Model._fast_decode = _fast_decode_impl
 
 
-def _generate_run_impl(self, last_tokens, first_pos, mems, n_steps, temperature, top_k, invalid_slices, sparse=None):
+def _generate_run_impl(self, last_tokens, first_pos, mems, n_steps, temperature, top_k, invalid_slices, sparse=None,
+                       row_pad=None):
     """n_steps sampled tokens in a row on the K|V cache — the inner loop of generation/sampling.py:147-183 for a
     stretch of the template that is all 'generate' slots — with the sampling tail inside the replayed CUDA graph
     (mpu/decode.py sample_run).  Returns None when the fast path does not apply, else
     (tokens [b, n_steps], summed log-probabilities [b], mems).
     sparse = dict(n_img=<image vocabulary size>, tokens=<[b, t + 1] all tokens so far>) runs the stretch with
     is_sparse == 2 semantics (mpu/sparse_transformer.py:498-520, :591-600, :727-750): pivots + trailing window per layer per
-    token, chosen on the device (cv_sparse_plan) instead of Python's random.sample — same distribution, other stream."""
+    token, chosen on the device (cv_sparse_plan) instead of Python's random.sample — same distribution, other stream.
+    first_pos is one position for every row, or one per row (a sequence or 1-D tensor of b positions).
+    row_pad (int32 [b] on the device, from mpu/kv_cache.py assemble): row i of `mems` holds mems[0].size(1) - row_pad[i]
+    tokens — rows of prompts of different lengths in one run (not with sparse)."""
     tr = self.transformer
     b = last_tokens.shape[0]
     if (not mems or tr.mems_mode != 'kv' or tr.max_memory_length <= 0 or torch.is_grad_enabled()
@@ -158,12 +162,16 @@ def _generate_run_impl(self, last_tokens, first_pos, mems, n_steps, temperature,
     if runner is None:
         runner = caches.runner = DecodeRunner(self, caches,
                                               use_graph=os.environ.get('COGVIEW_B200_CUDA_GRAPH', '1') != '0')
-    pos = torch.full((b, 1), int(first_pos), dtype=torch.long, device=last_tokens.device)
+    if torch.is_tensor(first_pos) or isinstance(first_pos, (list, tuple)):
+        pos = torch.as_tensor(first_pos, dtype=torch.long).to(last_tokens.device).reshape(b, 1)
+    else:
+        pos = torch.full((b, 1), int(first_pos), dtype=torch.long, device=last_tokens.device)
     # sparse inference: cv_sparse_plan is written for at most 16 sequences
-    if sparse is not None and (b > ops.DECODE_SMALL_MAX_BATCH or tr.max_memory_length > 4096 or runner.persistent):
+    if sparse is not None and (b > ops.DECODE_SMALL_MAX_BATCH or tr.max_memory_length > 4096 or runner.persistent
+                               or row_pad is not None):
         return None
     new_tokens, logp = runner.sample_run(last_tokens.reshape(b, 1), pos, caches.t, n_steps, temperature, top_k,
-                                         invalid_slices, sparse=sparse)
+                                         invalid_slices, sparse=sparse, row_pad=row_pad)
     return new_tokens, logp, caches.views()
 
 

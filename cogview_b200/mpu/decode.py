@@ -6,7 +6,8 @@ it (one new token per sequence, `mems` returned by the previous call, mems_mode 
 Two device paths:
   * default: one kernel per operation (cv_attn_decode between cv_linear_small_m / cv_ln_pair_small_m at batch <= 16,
     cv_linear_mid_m / cv_ln_pair_mid_m at batch 17..64), CUDA-graph captured; in generation runs followed by ONE
-    sampling kernel (cv_sample_topk) inside the same graph.
+    sampling kernel (cv_sample_topk) inside the same graph.  In ragged mode (rows from prompts of different lengths,
+    row_pad given) the attention is cv_attn_decode_ragged: row i holds cur_len - row_pad[i] cached tokens.
   * COGVIEW_B200_PERSISTENT=1 and batch <= 8: the whole step — embedding, 48 Sandwich-LN layers, final LayerNorm,
     logits — is ONE persistent kernel (cv_decode_step, csrc/decode_step.cu: bulk-copy weight stream through a
     shared-memory byte ring, register-resident residual stream, grid barriers between the dependency points).  Parity-
@@ -38,7 +39,10 @@ class DecodeRunner:
         self.pos = torch.zeros((self.b, 1), dtype=torch.int64, device=dev)
         self.cur_len = torch.zeros(1, dtype=torch.int32, device=dev)
         self.step_logits = None          # output buffer of the step (static: graphs write into it)
-        self.graph = None
+        # ragged mode: row i holds cur_len - row_pad[i] cached tokens; captured graphs read this static buffer
+        self.ragged = False
+        self.row_pad = torch.zeros(self.b, dtype=torch.int32, device=dev)
+        self.step_graphs = {}            # ragged (bool) -> captured step
         self.use_graph = use_graph
         assert self.b <= ops.DECODE_MAX_BATCH
         # which pair of kernels runs the linears and the Sandwich-LN glue is a property of the batch size
@@ -93,7 +97,7 @@ class DecodeRunner:
             self.workspace = ops.decode_step_workspace(self.h, self.heads, dev)
             self.step_logits = torch.empty((self.b, self.wte.shape[0]), dtype=torch.float32, device=dev)
         # captured graphs hold the old pointers
-        self.graph = None
+        self.step_graphs = {}
         self.sample_graphs = {}
 
     def _check_params(self):
@@ -112,7 +116,7 @@ class DecodeRunner:
             self.len64 = torch.zeros((1, 1), dtype=torch.int64, device=dev)
 
     def _run(self):
-        if self.persistent and self.sparse is None:
+        if self.persistent and self.sparse is None and not self.ragged:
             ops.decode_step(self.layer_table, len(self.params), self.heads, self.eps, self.fl[2], self.wte, self.wpe,
                             self.fl[0], self.fl[1], self.ids, self.pos, self.cur_len, self.caches.buf,
                             self.step_logits, self.workspace)
@@ -146,7 +150,8 @@ class DecodeRunner:
                 ctx = ops.attn_decode_gather(qkv, self.caches.buf[i], heads, self.cur_len, self.key_idx[i], self.n_keys,
                                              nsplit=self.nsplit)
             else:
-                ctx = ops.attn_decode(qkv, self.caches.buf[i], heads, cur_len_dev=self.cur_len, nsplit=self.nsplit)
+                ctx = ops.attn_decode(qkv, self.caches.buf[i], heads, cur_len_dev=self.cur_len, nsplit=self.nsplit,
+                                      row_pad=self.row_pad if self.ragged else None)
             attn_out = self.linear(ctx, wd, bd, absmax=s[0:1])
             # y = x + LN3(attn_out);  xn2 = LN2(y)
             x, xn2 = self.ln_pair(x, attn_out, s[0:1], (g3, b3), (g2, b2), self.eps)
@@ -159,18 +164,28 @@ class DecodeRunner:
             self.step_logits = torch.empty((b, self.wte.shape[0]), dtype=torch.float32, device=self.ids.device)
         return self.linear(xf, self.wte, out=self.step_logits)
 
-    def step(self, ids, pos, t):
-        """ids, pos: [b, 1] int64; t: tokens already cached.  Returns logits [b, V] fp32 (a static buffer that the
-        next step overwrites; the sampling graphs never modify it)."""
+    def _set_rows(self, row_pad):
+        """Uniform (row_pad None) or ragged mode for the next step or run."""
+        self.ragged = row_pad is not None
+        if self.ragged:
+            assert row_pad.shape == (self.b,)
+            self.row_pad.copy_(row_pad)
+
+    def step(self, ids, pos, t, row_pad=None):
+        """ids, pos: [b, 1] int64; t: tokens already cached (in ragged mode, in the longest row; row i holds
+        t - row_pad[i]).  Returns logits [b, V] fp32 (a static buffer that the next step overwrites; the sampling
+        graphs never modify it)."""
         if self.params is None or t <= self.last_t:      # a new sequence: make sure the weights are the live ones
             self._check_params()
         self.last_t = t
+        self._set_rows(row_pad)
         self.ids.copy_(ids)
         self.pos.copy_(pos)
         self.cur_len.fill_(t)
+        graph = self.step_graphs.get(self.ragged)
         if not self.use_graph:
             self._run()
-        elif self.graph is None:
+        elif graph is None:
             side = torch.cuda.Stream()
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
@@ -179,14 +194,14 @@ class DecodeRunner:
             torch.cuda.current_stream().wait_stream(side)
             from .._lib import lib
             before = lib().cv_launch_count()
-            self.graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self.graph):
+            graph = self.step_graphs[self.ragged] = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
                 self._run()
             self.graph_launches = int(lib().cv_launch_count() - before)
-            self.graph.replay()
+            graph.replay()
             self.replays += 1
         else:
-            self.graph.replay()
+            graph.replay()
             self.replays += 1
         return self.step_logits
 
@@ -237,16 +252,20 @@ class DecodeRunner:
             self.len64.fill_(t)
             self.plan_err.zero_()
 
-    def sample_run(self, ids, pos, t, n_steps, temperature, top_k, invalid_slices, sparse=None):
+    def sample_run(self, ids, pos, t, n_steps, temperature, top_k, invalid_slices, sparse=None, row_pad=None):
         """n_steps tokens starting from `ids` ([b, 1], at positions `pos`, t tokens cached).  One graph replay per
         token.  Returns (tokens [b, n_steps] int64, summed log-probabilities [b] fp32).
-        sparse: None, or dict(n_img=..., tokens=[b, t + 1] every token so far) for is_sparse == 2."""
+        sparse: None, or dict(n_img=..., tokens=[b, t + 1] every token so far) for is_sparse == 2.
+        row_pad: None, or int32 [b] on the device: row i holds t - row_pad[i] cached tokens (ragged mode; not with
+        sparse)."""
+        assert sparse is None or row_pad is None
         self._check_params()
         self.last_t = t + n_steps
         vocab = self.model.word_embeddings.weight.shape[0]
         key = (float(temperature), int(top_k), tuple(sl.indices(vocab)[:2] for sl in invalid_slices),
-               None if sparse is None else int(sparse['n_img']))
+               None if sparse is None else int(sparse['n_img']), row_pad is not None)
         assert n_steps <= self.out_buf.shape[1]
+        self._set_rows(row_pad)
         self.sparse = None
         if sparse is not None:
             self._ensure_sparse_buffers()

@@ -84,9 +84,8 @@ def _make_room(owner, pool, b):
         del pool[k]
 
 
-def prepare(owner, mems, b, sq):
-    """Find (or build) the cache that `mems` refers to and get it ready for sq more tokens.  One cache (and its
-    captured decode graph) is kept per batch size and reused across sequences, within POOL_BYTE_BUDGET."""
+def _pooled(owner, b):
+    """(pool, the pooled cache of batch size b or None); room for a new one is made when there is none."""
     dev = owner.position_embeddings.weight.device
     pool = owner.__dict__.setdefault('_kv_pool', {})
     c = pool.get(b)
@@ -95,6 +94,13 @@ def prepare(owner, mems, b, sq):
         del pool[b]
     if c is None:
         _make_room(owner, pool, b)
+    return pool, c, dev
+
+
+def prepare(owner, mems, b, sq):
+    """Find (or build) the cache that `mems` refers to and get it ready for sq more tokens.  One cache (and its
+    captured decode graph) is kept per batch size and reused across sequences, within POOL_BYTE_BUDGET."""
+    pool, c, dev = _pooled(owner, b)
     if not mems:
         if c is None:
             c = _Caches(owner, b, dev)
@@ -110,3 +116,31 @@ def prepare(owner, mems, b, sq):
     owner._kv = c
     c.begin(sq)
     return c
+
+
+def assemble(owner, caption_mems, rows, run):
+    """The cache of one decode batch whose rows come from prompts of different lengths.  caption_mems[c] is prompt
+    c's `mems` at batch 1 (len_c tokens, as GPT2Model.forward returned them); its K|V fills slots [0, len_c) of the
+    next rows[c] rows of the pooled cache of batch size sum(rows).  Returns (mems of that batch, t = max(len_c) tokens
+    long, row_pad int32 [b] on the device = t - len_c of every row): the decode continues row i at its own length
+    t - row_pad[i] (DecodeRunner's ragged mode).  Slots past a row's own length are left as they were."""
+    lens = [m[0].size(1) for m in caption_mems]
+    t = max(lens)
+    if t + run > owner.max_memory_length:
+        raise NotImplementedError('KV-cache overflow: longest prompt %d + %d new tokens > max_memory_length %d'
+                                  % (t, run, owner.max_memory_length))
+    b = sum(rows)
+    pool, c, dev = _pooled(owner, b)
+    if c is None:
+        c = _Caches(owner, b, dev)
+    r0 = 0
+    for mems, n, ln in zip(caption_mems, rows, lens):
+        assert len(mems) == c.L + 1 and mems[0].size(0) == 1
+        for i in range(c.L):
+            c.buf[i, r0:r0 + n, :ln].copy_(mems[i].expand(n, -1, -1))
+        r0 += n
+    c.t = t
+    pool[b] = c
+    owner._kv = c
+    row_pad = torch.tensor([t - ln for ln, n in zip(lens, rows) for _ in range(n)], dtype=torch.int32, device=dev)
+    return [c.buf[i, :, :t] for i in range(c.L)] + [c.dummy[:, :t]], row_pad

@@ -326,10 +326,12 @@ def linear_mid_m(x, w, bias=None, *, act=ACT_NONE, out_dtype=torch.bfloat16, abs
     return _decode_linear("cv_linear_mid_m", x, w, bias, act, out_dtype, absmax, out)
 
 
-def attn_decode(qkv, cache, heads, *, cur_len=None, cur_len_dev=None, nsplit=1, out=None, workspace=None):
+def attn_decode(qkv, cache, heads, *, cur_len=None, cur_len_dev=None, nsplit=1, out=None, workspace=None,
+                row_pad=None):
     """qkv: [b, 3h] bf16; cache: [b, max_len, 2h] bf16 (K|V); appends the new token at cur_len and returns
-    the attention context [b, h] bf16."""
-    require_cuda(qkv, cache)
+    the attention context [b, h] bf16.  row_pad (int32 [b] on the device, 0 <= row_pad[i] <= cur_len): row i holds
+    cur_len - row_pad[i] cached tokens and appends there (cv_attn_decode_ragged)."""
+    require_cuda(qkv, cache, row_pad)
     b, h3 = qkv.shape
     h = h3 // 3
     assert qkv.is_contiguous() and cache.stride(2) == 1 and cache.stride(1) == 2 * h and cache.shape[2] == 2 * h
@@ -338,9 +340,15 @@ def attn_decode(qkv, cache, heads, *, cur_len=None, cur_len_dev=None, nsplit=1, 
     if nsplit > 1 and workspace is None:
         workspace = torch.empty(lib().cv_attn_decode_workspace_bytes(b, heads, nsplit) // 4, dtype=torch.float32,
                                 device=qkv.device)
-    rc = lib().cv_attn_decode(ptr(qkv), ptr(cache), cache.stride(0), ptr(cur_len_dev),
-                              -1 if cur_len is None else int(cur_len), ptr(out), ptr(workspace), b, heads, 64,
-                              cache.shape[1], nsplit, stream_ptr())
+    cl = -1 if cur_len is None else int(cur_len)
+    if row_pad is not None:
+        assert row_pad.dtype == torch.int32 and row_pad.is_contiguous() and row_pad.numel() == b
+        rc = lib().cv_attn_decode_ragged(ptr(qkv), ptr(cache), cache.stride(0), ptr(cur_len_dev), cl, ptr(row_pad),
+                                         ptr(out), ptr(workspace), b, heads, 64, cache.shape[1], nsplit, stream_ptr())
+        check(rc, "cv_attn_decode_ragged")
+        return out
+    rc = lib().cv_attn_decode(ptr(qkv), ptr(cache), cache.stride(0), ptr(cur_len_dev), cl, ptr(out), ptr(workspace), b,
+                              heads, 64, cache.shape[1], nsplit, stream_ptr())
     check(rc, "cv_attn_decode")
     return out
 

@@ -233,6 +233,14 @@ int64_t cv_attn_decode_workspace_bytes(int b, int heads, int nsplit);
 int cv_attn_decode(const void* qkv, void* cache, int64_t cache_batch_stride, const int* cur_len_dev, int cur_len,
                    void* out, float* workspace, int b, int heads, int head_dim, int max_len, int nsplit,
                    void* stream);
+/* cv_attn_decode with a cache length per sequence, for a batch whose rows come from prompts of different lengths:
+ * row_pad is device int32 [b], and row b holds t_b = cur_len - row_pad[b] cached tokens (cur_len from *cur_len_dev
+ * when non-NULL, else cur_len: the longest row).  Row b attends over its keys 0..t_b, the new token last, and appends
+ * its K|V at slot t_b; slots above t_b are neither read nor written.  Contract: 0 <= row_pad[b] <= cur_len and
+ * t_b < max_len.  With row_pad all zero, out and cache are bit-identical to cv_attn_decode at the same nsplit. */
+int cv_attn_decode_ragged(const void* qkv, void* cache, int64_t cache_batch_stride, const int* cur_len_dev, int cur_len,
+                          const int* row_pad, void* out, float* workspace, int b, int heads, int head_dim, int max_len,
+                          int nsplit, void* stream);
 /* Sparse inference (is_sparse == 2, mpu/sparse_transformer.py:498-520, :591-600, :727-750) without the host:
  *   cv_sparse_plan: the key index list of one decode step for EVERY layer: idx [num_layers, b, nmax] int32, *n_dev = its
  *     length.  Per (layer, sequence): every text position before the trailing window (is_txt [b, max_len] uint8 marks
