@@ -5,7 +5,7 @@ through the VQ-VAE.  Text <-> string conversion (sentencepiece) and image file I
 import torch
 
 from . import vqvae
-from .generation.magnify import magnify
+from .generation.magnify import magnify, magnify_batch
 from .generation.sampling import (add_interlacing_beam_marks, filling_sequence, filling_sequences, get_tokenizer,
                                   inverse_prompt_score)
 
@@ -155,6 +155,34 @@ def super_resolution(model, vq_model, args, seq, fill=filling_sequence, decode=N
             imgs.append(torch.nn.functional.interpolate(src, size=(512, 512)))
         imgs.append(decode(codes.view(1, 64, 64)))
     return codes, torch.cat(imgs, dim=0)
+
+
+def super_resolution_batch(model, vq_model, args, seqs, fill=filling_sequences, decode=None):
+    """super_resolution for many images: `seqs` is a list of filled 'super-resolution' templates, one per image (their
+    text lengths may differ).  Images are magnified in groups of at most args.max_inference_batch_size by
+    magnify_batch, whose `fill` runs each window of a group as one decode batch (filling_sequences: the given stretches
+    of every window go through GPT2Model.chunk_run, the generated ones through the ragged decode graph); each
+    magnified grid is then decoded by the VQ-VAE.  A group of one image, or a group whose templates cannot share a
+    batch (filling_sequences falls back to filling_sequence per template, e.g. COGVIEW_B200_FAST_DECODE=0), gives
+    what super_resolution gives.  Rows of a batch match solo runs within bf16 tolerance, not bit for bit (the abs-max
+    LayerNorm scales are taken over the whole batch).  Returns (codes [N, 4096], images [N, 3, 512, 512])."""
+    decode = decode or (lambda codes: vqvae.code2img(vq_model, codes))
+    tok = get_tokenizer(args)
+    mbz = max(1, args.max_inference_batch_size)
+    codes = []
+    model.eval()
+    with torch.no_grad():
+        for g0 in range(0, len(seqs), mbz):
+            group = seqs[g0:g0 + mbz]
+            if len(group) == 1:
+                codes.append(magnify(model, tok, group[0][-1024:], group[0][:-1024], args,
+                                     fill=lambda m, s, a, **kw: fill(m, [s], a)[0]))
+                continue
+            src = torch.stack([seq[-1024:] for seq in group])
+            codes.append(magnify_batch(model, tok, src, [seq[:-1024] for seq in group], args, fill=fill))
+        codes = torch.cat(codes, dim=0)
+        imgs = torch.cat([decode(c.view(1, 64, 64)) for c in codes], dim=0)
+    return codes, imgs
 
 
 def post_selection_rows(rows, text, tokenizer=None):

@@ -314,38 +314,172 @@ def _batch_plan(model, tmpls, args, tokenizer):
     return plans, ok
 
 
+def _stretches(tmpl, C, tokenizer):
+    """The part of a template after its context C as (structure, given, slices): structure is the tuple of
+    (given run length, generate run length, beam count) pairs in order (the first given run is empty: the context
+    ends where the first generate slot starts) followed by the length of a trailing given run; given[s] the provided
+    tokens before generate stretch s (given[-1]: the trailing ones); slices[s] the invalid vocabulary slices in force
+    at generate stretch s, as filling_sequence tracks them."""
+    _, _, inv = _scan_context(tmpl, tokenizer)
+    structure, given, slices = [], [], []
+    i, n, g0 = C, len(tmpl), C
+    while i < n:
+        g0 = i
+        while i < n and tmpl[i] >= 0:
+            inv = _slices_after(tokenizer, tmpl[i], inv)
+            i += 1
+        if i == n:
+            break
+        nb = tmpl[i]
+        k0 = i
+        while i < n and tmpl[i] == nb:
+            i += 1
+        structure.append((k0 - g0, i - k0, -nb))
+        given.append(tmpl[g0:k0])
+        slices.append(inv)
+    given.append(tmpl[g0:] if i == n and g0 < n and tmpl[n - 1] >= 0 else [])
+    structure.append(len(given[-1]))
+    return tuple(structure), given, slices
+
+
+def _stretch_plan(model, tmpls, args, tokenizer):
+    """Per template (context length, [ROI2] offset, (structure, given, slices) of _stretches), and whether
+    filling_sequences can run all of them as one decode batch with given stretches between the generate stretches
+    (super-resolution windows: each 32-code line is given codes, then generated ones): every template has at least
+    two generate stretches, all share one structure (the same given / generate run lengths in the same order, one
+    beam each) and the invalid slices at every generate stretch; the given tokens and the context length are each
+    template's own.  Plus the conditions of _batch_plan: dense attention on the K|V cache without nucleus sampling,
+    at most ops.DECODE_MAX_BATCH rows, the longest context plus the rest of the template within max_memory_length,
+    the graph-replayed decode path on."""
+    from .. import ops
+    plans, keys = [], set()
+    ok = (getattr(args, 'is_sparse', 0) == 0 and args.top_p == 0.0 and hasattr(model, 'generate_run')
+          and hasattr(model, 'chunk_run') and not torch.is_grad_enabled())
+    for tmpl in tmpls:
+        C, offset, _ = _scan_context(tmpl, tokenizer)
+        st = _stretches(tmpl, C, tokenizer)
+        plans.append((C, offset, st))
+        structure, _, slices = st
+        keys.add((structure, tuple(tuple((sl.start, sl.stop) for sl in inv) for inv in slices)))
+        ok = ok and C > 0 and len(structure) >= 3 and all(nb == 1 for _, _, nb in structure[:-1])
+    tr = getattr(model, 'transformer', None)
+    rows = len(tmpls)
+    ok = (ok and len(keys) == 1 and tr is not None and getattr(tr, 'mems_mode', None) == 'kv'
+          and rows <= ops.DECODE_MAX_BATCH and ops.decode_batch_supported(rows, tr.hidden_size)
+          and max(p[0] for p in plans) + len(tmpls[0]) - plans[0][0] - 1 <= tr.max_memory_length
+          and _os.environ.get('COGVIEW_B200_FAST_DECODE', '1') != '0'
+          and _os.environ.get('COGVIEW_B200_GRAPH_SAMPLING', '1') != '0')
+    return plans, ok
+
+
+def _row_positions(pos, offsets):
+    """Absolute positions [b, n] -> model position ids: positions after a row's [ROI2] restart from it
+    (position_ids[position_ids > offset] -= offset, per row)."""
+    off = torch.as_tensor(offsets, dtype=torch.long, device=pos.device).view(-1, 1).expand_as(pos)
+    return torch.where(pos > off, pos - off, pos)
+
+
+def _fill_interleaved(model, seqs, tmpls, plans, args, tokenizer):
+    """filling_sequences for templates that passed _stretch_plan: one row per template.  Each context is prefilled
+    alone and its first generated token drawn as filling_sequence draws it; its cache goes straight into its row of
+    the batch cache (kv_cache.assemble_rows, row_pad); then per generate stretch: the pending sampled token plus the given run go
+    through GPT2Model.chunk_run (in pieces of at most ops.ATTN_CHUNK_MAX tokens), the stretch's first slot is drawn
+    from its logits, and the rest of the stretch runs through generate_run on the ragged decode graph."""
+    from .. import ops
+    from ..mpu import kv_cache
+    device = seqs[0].device
+    roi2 = tokenizer['[ROI2]']
+    structure, _, slices = plans[0][2]
+    ctx = [p[0] for p in plans]
+    offsets = [p[1] for p in plans]
+    out = [seq.clone().view(1, -1) for seq in seqs]
+    last = []
+
+    def prefill(r):
+        tokens, attention_mask, position_ids = get_batch(seqs[r][:ctx[r]], device, args)
+        position_ids = position_ids.clone()
+        position_ids[position_ids > offsets[r]] -= offsets[r]
+        logits, *mems = model(tokens, position_ids, attention_mask, None, None, 0)
+        last.append(torch.multinomial(_next_token_probs(logits, slices[0], args), num_samples=1))
+        return mems
+    mems, row_pad = kv_cache.assemble_rows(model.transformer, ctx, [1] * len(seqs), len(tmpls[0]) - ctx[0] - 1,
+                                           prefill)
+    last = torch.cat(last, dim=0)
+    ctx_t = torch.tensor(ctx, dtype=torch.long, device=device).view(-1, 1)
+    rel = 0                                                  # template slot (after the context) of `last`
+    for s, (g, k, _) in enumerate(structure[:-1]):
+        if s > 0:
+            given = torch.tensor([p[2][1][s] for p in plans], dtype=torch.long, device=device)
+            for r, p in enumerate(plans):                    # a given [ROI2] restarts that row's positions
+                for e, tok in enumerate(p[2][1][s]):
+                    if tok == roi2:
+                        offsets[r] = ctx[r] + rel + 1 + e
+            chunk = torch.cat((last.to(device), given), dim=1)
+            pos = _row_positions(ctx_t + torch.arange(rel, rel + g + 1, device=device).view(1, -1), offsets)
+            for c0 in range(0, g + 1, ops.ATTN_CHUNK_MAX):
+                res = model.chunk_run(chunk[:, c0:c0 + ops.ATTN_CHUNK_MAX], pos[:, c0:c0 + ops.ATTN_CHUNK_MAX],
+                                      mems, row_pad)
+                if res is None:
+                    raise RuntimeError('filling_sequences: the chunk of %d rows was refused' % chunk.shape[0])
+                logits, mems = res
+            rel += g + 1
+            last = torch.multinomial(_next_token_probs(logits.unsqueeze(1), slices[s], args), num_samples=1)
+        for r, o in enumerate(out):
+            o[0, ctx[r] + rel] = last[r, 0]
+        if k > 1:
+            first_pos = _row_positions(ctx_t + rel, offsets).view(-1)
+            res = model.generate_run(last, first_pos, mems, k - 1, args.temperature, args.top_k, slices[s],
+                                     row_pad=row_pad)
+            if res is None:
+                raise RuntimeError('filling_sequences: the decode batch of %d rows was refused' % last.shape[0])
+            new_tokens, _, mems = res
+            for r, o in enumerate(out):
+                o[0, ctx[r] + rel + 1:ctx[r] + rel + k] = new_tokens[r].to(device)
+            last = new_tokens[:, -1:]
+        rel += k - 1
+    return out
+
+
 def filling_sequences(model, seqs, args):
     """filling_sequence for several templates (1-D LongTensors, e.g. one per caption) at once: returns one token tensor
     [nb, len(seq_c)] per template.  Each context is run through the model on its own (batch 1) and its nb first tokens
     are drawn as filling_sequence draws them; then the generate slots of all rows run as ONE decode batch (DecodeRunner
-    in ragged mode: every row continues at its own context length and position).  Templates that cannot share a batch
-    (see _batch_plan) are filled one by one with filling_sequence, as is a single template.
-    The abs-max LayerNorm scales of the decode step are taken over the whole batch, so a template's rows match a run
-    of that template alone within bf16 tolerance, not bit for bit."""
+    in ragged mode: every row continues at its own context length and position).  Templates that interleave given
+    and generated stretches with one beam each (super-resolution windows, see _stretch_plan) share a batch too: the
+    given stretches go through GPT2Model.chunk_run, every row at its own cache length.  Templates that cannot share a
+    batch (see _batch_plan and _stretch_plan) are filled one by one with filling_sequence, as is a single template.
+    The abs-max LayerNorm scales of the decode step and of the chunk are taken over the whole batch, so a template's
+    rows match a run of that template alone within bf16 tolerance, not bit for bit."""
     if len(seqs) == 1:
         return [filling_sequence(model, seqs[0], args)]
     tokenizer = get_tokenizer(args)
     tmpls = [seq.tolist() for seq in seqs]
     plans, ok = _batch_plan(model, tmpls, args, tokenizer)
     if not ok:
+        splans, sok = _stretch_plan(model, tmpls, args, tokenizer)
+        if sok:
+            return _fill_interleaved(model, seqs, tmpls, splans, args, tokenizer)
         return [filling_sequence(model, seq, args) for seq in seqs]
     from ..mpu import kv_cache
     device = seqs[0].device
-    prefixes, caption_mems, first_pos = [], [], []
-    for seq, tmpl, (C, offset, nb, n_gen) in zip(seqs, tmpls, plans):
-        _, _, invalid_slices = _scan_context(tmpl, tokenizer)
-        tokens, attention_mask, position_ids = get_batch(seq[:C], device, args)
+    prefixes, first_pos = [], []
+    _, _, invalid_slices = _scan_context(tmpls[0], tokenizer)     # shared by all templates (_batch_plan)
+
+    def prefill(c):
+        C, offset, nb, _ = plans[c]
+        tokens, attention_mask, position_ids = get_batch(seqs[c][:C], device, args)
         position_ids = position_ids.clone()
         position_ids[position_ids > offset] -= offset
         logits, *mems = model(tokens, position_ids, attention_mask, None, None, 0)
-        # the batch-1 cache is reused by the next prompt's forward: keep a copy of this prompt's K|V
-        caption_mems.append([m.clone() for m in mems])
         probs = _next_token_probs(logits, invalid_slices, args)
         prev = torch.multinomial(probs, num_samples=nb, replacement=True) if nb > 1 else torch.multinomial(probs, 1)
         prefixes.append(torch.cat((tokens.expand(nb, -1), prev.view(nb, 1)), dim=1))
-        first_pos += [C - offset if C > offset else C] * nb
+        first_pos.extend([C - offset if C > offset else C] * nb)
+        return mems
     run = plans[0][3] - 1
-    mems, row_pad = kv_cache.assemble(model.transformer, caption_mems, [p[2] for p in plans], run)
+    # each prompt's K|V goes into its rows of the batch cache before the next prompt reuses the batch-1 cache
+    mems, row_pad = kv_cache.assemble_rows(model.transformer, [p[0] for p in plans], [p[2] for p in plans], run,
+                                           prefill)
     last = torch.cat([p[:, -1:] for p in prefixes], dim=0)
     res = model.generate_run(last, first_pos, mems, run, args.temperature, args.top_k, invalid_slices,
                              row_pad=row_pad)

@@ -178,6 +178,54 @@ def _generate_run_impl(self, last_tokens, first_pos, mems, n_steps, temperature,
 GPT2Model.generate_run = _generate_run_impl
 
 
+def _chunk_run_impl(self, tokens, position_ids, mems, row_pad=None):
+    """n given tokens per row on the K|V cache in one eager pass — the model call generation/sampling.py:147-151
+    makes for a template stretch of provided tokens (plus the last sampled one), for a batch whose rows sit at
+    different cache lengths.  tokens, position_ids: int64 [b, n] (positions per row: every row has its own [ROI2]
+    offset); mems: the pooled cache views of kv_cache.assemble or of a previous generate_run / chunk_run; row_pad:
+    int32 [b] on the device or None, row i holding mems[0].size(1) - row_pad[i] tokens.  The attention of every layer
+    is cv_attn_chunk_ragged (each row against its own prefix, the chunk's K|V appended at the row's own length); the
+    linears and LayerNorms are the general kernels over the b*n rows, and the abs-max LayerNorm scales are taken over
+    the whole batch — so a row matches the same tokens run alone through forward within bf16 tolerance, not bit for
+    bit.  Returns (last position's logits [b, V] fp32, mems): every row's length grows by n, row_pad is unchanged, so
+    a following generate_run(..., row_pad=row_pad) continues each row at its own length.  None when the call does
+    not qualify (no K|V-cache mems, autograd on, n outside 1..ops.ATTN_CHUNK_MAX, or cache overflow)."""
+    tr = self.transformer
+    b, n = tokens.shape
+    if (not mems or tr.mems_mode != 'kv' or tr.max_memory_length <= 0 or torch.is_grad_enabled()
+            or not 1 <= n <= ops.ATTN_CHUNK_MAX or mems[0].size(1) + n > tr.max_memory_length
+            or position_ids.shape != tokens.shape or mems[0].size(0) != b):
+        return None
+    t = mems[0].size(1)
+    heads = tr.num_attention_heads
+    nsplit = ops.attn_chunk_nsplit(b, heads, t + n, tokens.device)
+    work = None
+    if nsplit > 1:
+        work = torch.empty(ops.lib().cv_attn_chunk_workspace_bytes(b, heads, n, nsplit) // 4, dtype=torch.float32,
+                           device=tokens.device)
+
+    def chunk_attn(i, caches):
+        cache_i = caches.buf[i]
+
+        def attn(q):
+            # q is the first third of the packed QKV GEMM output [b, n, 3h]: the kernel reads q | k | v in place
+            qkv = q.as_strided((b, n, q.shape[2] * 3), (q.stride(0), q.stride(1), 1))
+            return ops.attn_chunk_ragged(qkv, cache_i, heads, t, row_pad, nsplit=nsplit, workspace=work)
+        return attn
+
+    wte, wpe = self.word_embeddings.weight, tr.position_embeddings.weight
+    am_x = ops.new_scalars(1, wte.device)
+    x = ops.embed_fwd(tokens, position_ids, _as_bf16(wte.detach()).contiguous(), _as_bf16(wpe.detach()).contiguous(),
+                      am_x)
+    y, mem_layers = tr.run_layers(x, am_x, b, n, 0, mems, chunk_attn=chunk_attn)
+    y = y.view(b, n, -1)[:, -1].contiguous()
+    logits = _LogitsFn.forward(_NoCtx(), y, wte.detach())
+    return logits, mem_layers
+
+
+GPT2Model.chunk_run = _chunk_run_impl
+
+
 class _NoCtx:
     def save_for_backward(self, *a):
         pass

@@ -61,8 +61,10 @@ class _Caches:
 
 # Caches of several batch sizes are kept so that a run that alternates between them (one prompt, then its beams)
 # does not re-allocate and re-capture; but at the 4B shape a 32-sequence and a 64-sequence cache together are 51 GB.
-# When the pooled caches would exceed this many bytes, those of the other batch sizes are dropped first.
-POOL_BYTE_BUDGET = 40 << 30
+# When the pooled caches would exceed this many bytes, those of the other batch sizes are dropped first.  It holds a
+# 64-row cache of the 4B shape at max_memory_length 1345 (super-resolution windows: 39.4 GiB) together with the batch-1
+# cache its prompts are prefilled in (0.6 GiB), so the two are not dropped and re-made in turn for every window.
+POOL_BYTE_BUDGET = 41 << 30
 
 
 def cache_bytes(owner, b):
@@ -81,6 +83,9 @@ def _make_room(owner, pool, b):
         total -= pool[k].buf.numel() * 2
         if getattr(owner, '_kv', None) is pool[k]:
             owner._kv = None
+        # the cache and its DecodeRunner refer to each other: break the cycle so that the cache's memory is returned
+        # now, not at the next garbage collection (a new cache of another size is about to be allocated)
+        pool[k].runner = None
         del pool[k]
 
 
@@ -143,4 +148,34 @@ def assemble(owner, caption_mems, rows, run):
     pool[b] = c
     owner._kv = c
     row_pad = torch.tensor([t - ln for ln, n in zip(lens, rows) for _ in range(n)], dtype=torch.int32, device=dev)
+    return [c.buf[i, :, :t] for i in range(c.L)] + [c.dummy[:, :t]], row_pad
+
+
+def assemble_rows(owner, lens, rows, run, prefill):
+    """assemble without holding every prompt's cache at once (super-resolution windows have contexts of ~800 tokens:
+    64 copies of such a batch-1 cache take as much memory as the batch cache itself).  prefill(c) runs prompt c at
+    batch 1 and returns its `mems` (lens[c] tokens); they are copied into the next rows[c] rows of the pooled cache of
+    batch size sum(rows) before the next prompt runs.  Same cache contents and return value as assemble."""
+    t = max(lens)
+    if t + run > owner.max_memory_length:
+        raise NotImplementedError('KV-cache overflow: longest prompt %d + %d new tokens > max_memory_length %d'
+                                  % (t, run, owner.max_memory_length))
+    b = sum(rows)
+    c, r0 = None, 0
+    for ci, (n, ln) in enumerate(zip(rows, lens)):
+        mems = prefill(ci)
+        assert mems[0].size(0) == 1 and mems[0].size(1) == ln
+        if c is None:           # after the first prompt, whose batch-1 cache is then already pooled
+            pool, c, dev = _pooled(owner, b)
+            if c is None:
+                c = _Caches(owner, b, dev)
+            pool[b] = c
+        for i in range(c.L):
+            c.buf[i, r0:r0 + n, :ln].copy_(mems[i].expand(n, -1, -1))
+        r0 += n
+    c.t = t
+    pool[b] = c
+    owner._kv = c
+    row_pad = torch.tensor([t - ln for ln, n in zip(lens, rows) for _ in range(n)], dtype=torch.int32,
+                           device=c.buf.device)
     return [c.buf[i, :, :t] for i in range(c.L)] + [c.dummy[:, :t]], row_pad

@@ -601,8 +601,10 @@ class GPT2ParallelTransformer(torch.nn.Module):
                          dim=-1)
 
     def run_layers(self, x, am_x, b, sq, sep, mems, word_embedding_weight=None, is_sparse=0, txt_indices_bool=None,
-                   img_indices_bool=None):
-        """x fp32 [b*sq, h].  Returns (final-LN output bf16 [b*sq, h], mem_layers list)."""
+                   img_indices_bool=None, chunk_attn=None):
+        """x fp32 [b*sq, h].  Returns (final-LN output bf16 [b*sq, h], mem_layers list).
+        chunk_attn (K|V-cache mode only): None, or a callable (layer index, caches) -> attention hook that reads the
+        layer's cache and appends the new tokens' K|V itself (rows at their own cache lengths, GPT2Model.chunk_run)."""
         from . import kv_cache
         h = self.hidden_size
         keep_mems = self.max_memory_length > 0
@@ -647,6 +649,8 @@ class GPT2ParallelTransformer(torch.nn.Module):
                 def gather_attn(q, cache_i=cache_i, pw_idx=pw_idx):
                     return ops.attn_gather(q, cache_i[:, :t_all], pw_idx, heads)
                 out, am_x = layer.fused_forward(x, am_x, b, sq, sep, kv=caches.appender(i), attn=gather_attn)
+            elif mode == 'kv' and chunk_attn is not None:
+                out, am_x = layer.fused_forward(x, am_x, b, sq, sep, attn=chunk_attn(i, caches))
             elif mode == 'kv':
                 out, am_x = layer.fused_forward(x, am_x, b, sq, sep, kv=caches.appender(i))
             elif mems:   # hidden-state memory: exact reference semantics

@@ -353,6 +353,42 @@ def attn_decode(qkv, cache, heads, *, cur_len=None, cur_len_dev=None, nsplit=1, 
     return out
 
 
+ATTN_CHUNK_MAX = 64      # tokens per row of one cv_attn_chunk_ragged call
+
+
+def attn_chunk_nsplit(b, heads, keys, device):
+    """Key splits per (row, head) for cv_attn_chunk_ragged: about four CTAs per SM in all (a CTA walks its key range
+    one 64-key tile at a time, so one or two CTAs per SM leave HBM idle), at least 128 keys each."""
+    sms = torch.cuda.get_device_properties(device).multi_processor_count
+    return max(1, min(16, -(-4 * sms // (b * heads)), -(-keys // 128)))
+
+
+def attn_chunk_ragged(qkv, cache, heads, cur_len, row_pad=None, *, nsplit=None, out=None, workspace=None):
+    """Attention of a chunk of n new tokens per row against that row's cached prefix, with the chunk's K|V appended
+    (cv_attn_chunk_ragged).  qkv: [b, n, 3h] bf16 (the QKV GEMM output, read in place); cache: [b, max_len, 2h] bf16
+    (K|V, row stride 2h); row_pad: int32 [b] on the device or None — row i holds cur_len - row_pad[i] cached tokens,
+    query j of row i attends keys 0 .. cur_len - row_pad[i] + j, and the chunk is written at slots
+    cur_len - row_pad[i] ... onwards.  Returns the context [b, n, h] bf16."""
+    require_cuda(qkv, cache, row_pad)
+    b, n, h3 = qkv.shape
+    h = h3 // 3
+    assert qkv.dtype == torch.bfloat16 and cache.dtype == torch.bfloat16 and qkv.is_contiguous()
+    assert cache.shape[0] == b and cache.stride(2) == 1 and cache.stride(1) == 2 * h and cache.shape[2] == 2 * h
+    if row_pad is not None:
+        assert row_pad.dtype == torch.int32 and row_pad.is_contiguous() and row_pad.numel() == b
+    if nsplit is None:
+        nsplit = attn_chunk_nsplit(b, heads, int(cur_len) + n, qkv.device)
+    if out is None:
+        out = torch.empty((b, n, h), dtype=torch.bfloat16, device=qkv.device)
+    if nsplit > 1 and workspace is None:
+        workspace = torch.empty(lib().cv_attn_chunk_workspace_bytes(b, heads, n, nsplit) // 4, dtype=torch.float32,
+                                device=qkv.device)
+    rc = lib().cv_attn_chunk_ragged(ptr(qkv), ptr(cache), cache.stride(0), int(cur_len), ptr(row_pad), ptr(out),
+                                    ptr(workspace), b, n, heads, 64, cache.shape[1], nsplit, stream_ptr())
+    check(rc, "cv_attn_chunk_ragged")
+    return out
+
+
 def sparse_plan(is_txt, cur_len_dev, num_layers, window, num_pivot, max_sequence_length, seed_dev, idx, n_dev, err):
     """Index plan of one sparse decode step for every layer (cv_sparse_plan).  is_txt: uint8 [b, max_len]; idx: int32
     [num_layers, b, nmax] (written); n_dev, err: int32 [1]; seed_dev: int64 [1]."""

@@ -241,6 +241,21 @@ int cv_attn_decode(const void* qkv, void* cache, int64_t cache_batch_stride, con
 int cv_attn_decode_ragged(const void* qkv, void* cache, int64_t cache_batch_stride, const int* cur_len_dev, int cur_len,
                           const int* row_pad, void* out, float* workspace, int b, int heads, int head_dim, int max_len,
                           int nsplit, void* stream);
+/* Ragged multi-token attention on the K|V cache (csrc/attn_chunk.cu): a chunk of n new tokens per sequence.
+ * qkv [b, n, 3h] bf16 is the packed QKV GEMM output (q | k | v per token, token-major, read in place); cache
+ * [b, max_len, 2h] bf16 (K | V) with batch stride cache_batch_stride elements; row_pad device int32 [b] or NULL.
+ * Row r holds t_r = cur_len - row_pad[r] cached tokens (t_r = cur_len for every row when row_pad is NULL).  Query i of
+ * row r (position t_r + i) attends keys 0 .. t_r + i: the row's cache, then the chunk causally; no sep.  Softmax of
+ * the scores scaled by 1/sqrt(64), as standard_attention.  The chunk's K|V is written at slots t_r .. t_r + n - 1 and
+ * nothing else in the cache is written.  out [b, n, h] bf16 (token-major, the out-projection GEMM's input).
+ * nsplit > 1 splits every row's keys over that many CTAs and merges them in a second kernel; it needs workspace of
+ * cv_attn_chunk_workspace_bytes(b, heads, n, nsplit) bytes.  Argument errors: head_dim != 64, n outside 1..64,
+ * cur_len + n > max_len, nsplit outside 1..64, misaligned pointers.  Contract (not checked, device data):
+ * 0 <= row_pad[r] <= cur_len. */
+int64_t cv_attn_chunk_workspace_bytes(int b, int heads, int n, int nsplit);
+int cv_attn_chunk_ragged(const void* qkv, void* cache, int64_t cache_batch_stride, int cur_len, const int* row_pad,
+                         void* out, float* workspace, int b, int n, int heads, int head_dim, int max_len, int nsplit,
+                         void* stream);
 /* Sparse inference (is_sparse == 2, mpu/sparse_transformer.py:498-520, :591-600, :727-750) without the host:
  *   cv_sparse_plan: the key index list of one decode step for EVERY layer: idx [num_layers, b, nmax] int32, *n_dev = its
  *     length.  Per (layer, sequence): every text position before the trailing window (is_txt [b, max_len] uint8 marks
