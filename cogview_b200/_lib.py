@@ -72,6 +72,10 @@ def _declare(lib):
         "cv_vq_argmin": [P, L, P, P, P, P, L, I, I, F, P],
         "cv_vq_lookup": [P, P, P, P, L, I, P],
         "cv_conv1x1_out3": [P, P, P, P, P, P, I, I, I, I, P],
+        "cv_conv_k4s2_wgrad": [P, P, P, P, I, I, I, I, I, P],
+        "cv_relu_mask_bf16": [P, P, L, P],
+        "cv_conv1x1_out3_bwd": [P, P, P, P, P, P, P, I, I, I, I, P],
+        "cv_vq_ema_stats": [P, P, L, I, I, P, P, P],
         "cv_embed_fwd": [P, P, P, P, P, P, I, I, F, U64, U32, P],
         "cv_embed_bwd": [P, P, P, P, P, I, I, F, U64, U32, P],
         "cv_dropout_mask": [P, L, F, U64, U32, P],
@@ -109,6 +113,10 @@ def _declare(lib):
     lib.cv_set_reserved_sms.restype = I
     lib.cv_colsum_workspace_bytes.argtypes = [I]
     lib.cv_colsum_workspace_bytes.restype = L
+    lib.cv_conv_k4s2_wgrad_workspace_bytes.argtypes = [I, I, I, I, I]
+    lib.cv_conv_k4s2_wgrad_workspace_bytes.restype = L
+    lib.cv_conv1x1_out3_bwd_workspace_bytes.argtypes = [I]
+    lib.cv_conv1x1_out3_bwd_workspace_bytes.restype = L
     for name, args in sigs.items():
         fn = getattr(lib, name)
         fn.argtypes = args

@@ -603,6 +603,61 @@ def conv1x1_out3(x, w, bias, scale, shift):
     return out
 
 
+def conv_k4s2_wgrad(s, g):
+    """Weight gradient of a k4 s2 p1 convolution: s [B, h, w, M], g [B, 2h, 2w, N] bf16 NHWC -> fp32 [M, N, 4, 4],
+    out[m, n, ky, kx] = sum_{b,y,x} s[b, y, x, m] g[b, 2y-1+ky, 2x-1+kx, n].  Conv2d: (s, g) = (dY, X) gives dW
+    [Cout, Cin, 4, 4]; ConvTranspose2d: (s, g) = (X, dY) gives dW [Cin, Cout, 4, 4]."""
+    require_cuda(s, g)
+    B, h, w, M = s.shape
+    N = g.shape[3]
+    assert s.is_contiguous() and g.is_contiguous() and s.dtype == torch.bfloat16 and g.dtype == torch.bfloat16
+    assert tuple(g.shape[:3]) == (B, 2 * h, 2 * w), "g must be the 2x map of s"
+    out = torch.empty((M, N, 4, 4), dtype=torch.float32, device=s.device)
+    ws = torch.empty(lib().cv_conv_k4s2_wgrad_workspace_bytes(B, h, w, M, N) // 4, dtype=torch.float32,
+                     device=s.device)
+    check(lib().cv_conv_k4s2_wgrad(ptr(s), ptr(g), ptr(out), ptr(ws), B, h, w, M, N, stream_ptr()),
+          "cv_conv_k4s2_wgrad")
+    return out
+
+
+def relu_mask_(dx, act):
+    """dx *= (act > 0) in place (ReLU backward from the saved ReLU output); both bf16, same shape."""
+    require_cuda(dx, act)
+    assert dx.shape == act.shape and dx.is_contiguous() and act.is_contiguous()
+    assert dx.dtype == torch.bfloat16 and act.dtype == torch.bfloat16
+    check(lib().cv_relu_mask_bf16(ptr(dx), ptr(act), dx.numel(), stream_ptr()), "cv_relu_mask_bf16")
+    return dx
+
+
+def conv1x1_out3_bwd(dr, x, w):
+    """Backward of conv1x1_out3 (scale 1, shift 0) after a ReLU: dr [B, 3, H, W] fp32, x [B, H, W, Cin] bf16 (the ReLU
+    output), w [3, Cin] fp32 -> (dx [B, H, W, Cin] bf16 masked by x > 0, dw [3, Cin] fp32, db [3] fp32)."""
+    require_cuda(dr, x, w)
+    B, H, W, Cin = x.shape
+    assert dr.shape == (B, 3, H, W) and dr.dtype == torch.float32 and dr.is_contiguous()
+    assert x.is_contiguous() and x.dtype == torch.bfloat16 and w.is_contiguous() and w.dtype == torch.float32
+    dx = torch.empty_like(x)
+    dw = torch.empty((3, Cin), dtype=torch.float32, device=x.device)
+    db = torch.empty(3, dtype=torch.float32, device=x.device)
+    ws = torch.empty(lib().cv_conv1x1_out3_bwd_workspace_bytes(Cin) // 4, dtype=torch.float32, device=x.device)
+    check(lib().cv_conv1x1_out3_bwd(ptr(dr), ptr(x), ptr(w), ptr(dx), ptr(dw), ptr(db), ptr(ws), B, H, W, Cin,
+                                    stream_ptr()), "cv_conv1x1_out3_bwd")
+    return dx, dw, db
+
+
+def vq_ema_stats(idx, z, n_embed):
+    """idx [rows] int64 codes, z [rows, dim] fp32 -> (counts [n_embed] fp32, embed_sum [dim, n_embed] fp32)."""
+    require_cuda(idx, z)
+    idx = idx.contiguous().view(-1)
+    rows, dim = z.shape
+    assert idx.numel() == rows and idx.dtype == torch.int64 and z.dtype == torch.float32 and z.is_contiguous()
+    counts = torch.empty(n_embed, dtype=torch.float32, device=z.device)
+    embed_sum = torch.empty((dim, n_embed), dtype=torch.float32, device=z.device)
+    check(lib().cv_vq_ema_stats(ptr(idx), ptr(z), rows, dim, n_embed, ptr(counts), ptr(embed_sum), stream_ptr()),
+          "cv_vq_ema_stats")
+    return counts, embed_sum
+
+
 def attn_gather(q, cache, idx, heads):
     """sparse_attention_inference: q [b, sq, h] view, cache [b, max_len, 2h] (K|V), idx [b, n] int64 -> [b, sq, h]."""
     require_cuda(q, cache, idx)

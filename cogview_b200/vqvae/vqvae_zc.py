@@ -2,12 +2,17 @@
 (`vqvae.api.new_model()`: channel=512, n_res_block=0, embed_dim=256, n_embed=8192, stride=6, simple=True): same
 class names, constructor arguments, parameter/buffer names (state_dict keys `enc_b.blocks.{0,2,4,6}`,
 `quantize_t.{embed,cluster_size,embed_avg}`, `dec.blocks.{0,2,4,6}`) and method signatures, on the inference
-paths `encode` (img -> codes) and `decode_code` (codes -> img).  Training of the VQ-VAE itself (EMA codebook
-updates, gumbel relaxation, vqvae_zc.py:55-83, :284-346) is outside the accelerated path and raises.
+paths `encode` (img -> codes) and `decode_code` (codes -> img), and in train() mode `forward` (img -> recon, diff)
+with the EMA codebook update (vqvae_zc.py:67-83) and a backward for every parameter.  The gumbel relaxations
+(continuous_relax=True, :55-64, :87-91, :284-346) are not accelerated and raise.
 
 Device layout: NHWC bf16 activations; the three stride-2 4x4 convolutions and the three transposed convolutions run
 as im2col-free wgmma implicit GEMMs (cv_conv2d_k4s2 / cv_conv_transpose2d_k4s2), the Cin=3 first conv as
-im2col + GEMM, the 1x1 convs as GEMMs, the quantiser as a 3-term bf16-split tensor-core GEMM + arg-min kernel."""
+im2col + GEMM, the 1x1 convs as GEMMs, the quantiser as a 3-term bf16-split tensor-core GEMM + arg-min kernel.
+Training: one autograd Function per network half (_EncoderFn, _DecoderFn) saves the bf16 ReLU outputs; data gradients
+run on the forward convolution kernels with the adjoint packing (the data gradient of Conv2d(k4, s2, p1) is
+ConvTranspose2d(k4, s2, p1) with the same weight, and the reverse) followed by the ReLU mask, weight gradients on
+cv_conv_k4s2_wgrad and the GEMM's wgrad operand modes, bias gradients on cv_colsum_bf16."""
 import torch
 from torch import nn
 
@@ -66,9 +71,10 @@ class Quantize(nn.Module):
         return self._cache.get("tables", [self.embed], build)
 
     def forward_(self, input, continuous_relax=False, temperature=1., hard=False):
-        if continuous_relax or self.training:
-            raise NotImplementedError('only the hard nearest-code inference path is accelerated (eval mode, '
-                                      'continuous_relax=False)')
+        if continuous_relax:
+            raise NotImplementedError('only the hard nearest-code path is accelerated (continuous_relax=False)')
+        if self.training:
+            return self._forward_train(input)
         flatten = input.reshape(-1, self.dim).float().contiguous()
         et, packed, e2 = self._tables()
         idx_parts = []
@@ -81,6 +87,33 @@ class Quantize(nn.Module):
         quantize = quant.view(*input.shape)
         diff = (quantize - input.float()).pow(2).mean()
         return quantize, diff, embed_ind
+
+    def _nearest(self, flatten):
+        et, packed, e2 = self._tables()
+        idx_parts = []
+        for r0 in range(0, flatten.shape[0], self.score_chunk_rows):
+            zc = flatten[r0:r0 + self.score_chunk_rows]
+            scores = ops.gemm(ops.vq_split3(zc), packed, out_dtype=torch.float32)
+            idx_parts.append(ops.vq_argmin(scores, e2, zc, et))
+        return torch.cat(idx_parts), et
+
+    def _forward_train(self, input):
+        """vqvae_zc.py:41-54, :67-86 (hard path): the code is chosen and looked up with the codebook as it was before
+        this step's EMA update; then cluster_size, embed_avg and embed are updated in place, in the reference's order."""
+        flatten = input.detach().reshape(-1, self.dim).float().contiguous()
+        embed_ind, et = self._nearest(flatten)
+        _, quant = ops.vq_lookup(embed_ind, et, want_bf16=False, want_f32=True)
+        quant = quant.view(*input.shape)
+        embed_onehot_sum, embed_sum = ops.vq_ema_stats(embed_ind, flatten, self.n_embed)
+        with torch.no_grad():
+            self.cluster_size.mul_(self.decay).add_(embed_onehot_sum, alpha=1 - self.decay)
+            self.embed_avg.mul_(self.decay).add_(embed_sum, alpha=1 - self.decay)
+            n = self.cluster_size.sum()
+            cluster_size = (self.cluster_size + self.eps) / (n + self.n_embed * self.eps) * n
+            self.embed.copy_(self.embed_avg / cluster_size.unsqueeze(0))
+        diff = (quant - input).pow(2).mean()
+        quantize = input + (quant - input).detach()        # straight-through estimator
+        return quantize, diff, embed_ind.view(*input.shape[:-1])
 
     def embed_code(self, embed_id):
         et, _, _ = self._tables()
@@ -116,8 +149,16 @@ class Encoder(nn.Module):
         return self._cache.get("enc", [b[0].weight, b[0].bias, b[2].weight, b[2].bias, b[4].weight, b[4].bias,
                                        b[6].weight, b[6].bias], build)
 
+    def _packed_bwd(self):
+        b = self.blocks
+        # the data gradient of Conv2d(k4, s2, p1) is ConvTranspose2d(k4, s2, p1) with the same weight tensor
+        return self._cache.get("enc_bwd", [b[2].weight, b[4].weight],
+                               lambda: dict(w2=_pack_convT(b[2].weight), w4=_pack_convT(b[4].weight)))
+
     def forward(self, input):
         """input: [B, 3, H, W] (normalised image) -> [B, H/8, W/8, embed_dim] fp32 (NHWC, as the reference returns)."""
+        if self.training:
+            return _EncoderFn.apply(input, self, *[t for m in self.blocks[0::2] for t in (m.weight, m.bias)])
         P = self._packed()
         B, _, H, W = input.shape
         ch = P['w0'].shape[0]
@@ -174,9 +215,100 @@ class Decoder(nn.Module):
             outs.append(ops.conv1x1_out3(x, P['w6'], P['b6'], one, zero))
         return outs[0] if len(outs) == 1 else torch.cat(outs)
 
+    def _packed_bwd(self):
+        b = self.blocks
+        # the data gradient of ConvTranspose2d(k4, s2, p1) is Conv2d(k4, s2, p1) with the same weight tensor
+        return self._cache.get("dec_bwd", [b[0].weight, b[2].weight, b[4].weight],
+                               lambda: dict(w0=_pack_conv(b[0].weight), w2=_pack_conv(b[2].weight),
+                                            w4=_pack_conv(b[4].weight)))
+
     def forward(self, input):
         """input: [B, C, h, w] (NCHW, as the reference) -> [B, 3, 8h, 8w]."""
+        if self.training:
+            return _DecoderFn.apply(input.permute(0, 2, 3, 1), self,
+                                    *[t for m in self.blocks[0::2] for t in (m.weight, m.bias)])
         return self.forward_nhwc(input.permute(0, 2, 3, 1).to(torch.bfloat16).contiguous())
+
+
+def _bias_grad(g2d):
+    return ops.colsum(g2d).float()
+
+
+class _EncoderFn(torch.autograd.Function):
+    """Encoder forward (the kernels of Encoder.forward in eval mode, without batch chunking) and its backward for the
+    eight parameters.  Saved: the first conv's im2col patches and the three bf16 ReLU outputs."""
+
+    @staticmethod
+    def forward(ctx, img, enc, *params):
+        P = enc._packed()
+        B, _, H, W = img.shape
+        ch = P['w0'].shape[0]
+        a0 = ops.im2col_k4s2_c3(img.detach().float().contiguous())
+        x1 = ops.gemm(a0, P['w0'], bias=P['b0'], act=ops.ACT_RELU).view(B, H // 2, W // 2, ch)
+        x2 = ops.conv2d_k4s2(x1, P['w2'], P['b2'], relu=True)
+        x3 = ops.conv2d_k4s2(x2, P['w4'], P['b4'], relu=True)
+        z = ops.gemm(x3.view(-1, ch), P['w6'], bias=P['b6'], out_dtype=torch.float32)
+        ctx.save_for_backward(a0, x1, x2, x3)
+        ctx.P, ctx.PT = P, enc._packed_bwd()
+        return z.view(B, H // 8, W // 8, -1)
+
+    @staticmethod
+    def backward(ctx, dz):
+        a0, x1, x2, x3 = ctx.saved_tensors
+        P, PT = ctx.P, ctx.PT
+        ch = x3.shape[-1]
+        dz = dz.to(torch.bfloat16).contiguous().view(-1, dz.shape[-1])               # [pixels, embed_dim]
+        dw6 = ops.gemm(dz, x3.view(-1, ch), a_mn_major=True, b_mn_major=True, out_dtype=torch.float32)
+        db6 = _bias_grad(dz)
+        g3 = ops.relu_mask_(ops.gemm(dz, P['w6'], b_mn_major=True), x3.view(-1, ch)).view(x3.shape)
+        dw4 = ops.conv_k4s2_wgrad(g3, x2)
+        db4 = _bias_grad(g3.view(-1, ch))
+        g2 = ops.relu_mask_(ops.conv_transpose2d_k4s2(g3, PT['w4'], None, relu=False), x2)
+        dw2 = ops.conv_k4s2_wgrad(g2, x1)
+        db2 = _bias_grad(g2.view(-1, ch))
+        g1 = ops.relu_mask_(ops.conv_transpose2d_k4s2(g2, PT['w2'], None, relu=False), x1).view(-1, ch)
+        # first conv through its im2col matrix: columns (ky * 4 + kx) * 3 + c of the 64 (48 used)
+        dw0 = ops.gemm(g1, a0, a_mn_major=True, b_mn_major=True, out_dtype=torch.float32)[:, :48]
+        dw0 = dw0.reshape(ch, 4, 4, 3).permute(0, 3, 1, 2).contiguous()
+        db0 = _bias_grad(g1)
+        return (None, None, dw0, db0, dw2, db2, dw4, db4, dw6.view(dw6.shape[0], ch, 1, 1), db6)
+
+
+class _DecoderFn(torch.autograd.Function):
+    """Decoder forward (the kernels of Decoder.forward_nhwc, without batch chunking) from NHWC fp32 quant and its
+    backward for the eight parameters and for quant.  Saved: the bf16 input and the three bf16 ReLU outputs."""
+
+    @staticmethod
+    def forward(ctx, quant_nhwc, dec, *params):
+        P = dec._packed()
+        dev = quant_nhwc.device
+        x0 = quant_nhwc.detach().to(torch.bfloat16).contiguous()
+        a1 = ops.conv_transpose2d_k4s2(x0, P['w0'], P['b0'], relu=True)
+        a2 = ops.conv_transpose2d_k4s2(a1, P['w2'], P['b2'], relu=True)
+        a3 = ops.conv_transpose2d_k4s2(a2, P['w4'], P['b4'], relu=True)
+        out = ops.conv1x1_out3(a3, P['w6'], P['b6'], torch.ones(3, device=dev), torch.zeros(3, device=dev))
+        ctx.save_for_backward(x0, a1, a2, a3)
+        ctx.P, ctx.PT = P, dec._packed_bwd()
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        x0, a1, a2, a3 = ctx.saved_tensors
+        P, PT = ctx.P, ctx.PT
+        ch = a3.shape[-1]
+        g3, dw6, db6 = ops.conv1x1_out3_bwd(dout.float().contiguous(), a3, P['w6'])
+        dw4 = ops.conv_k4s2_wgrad(a2, g3)
+        db4 = _bias_grad(g3.view(-1, ch))
+        g2 = ops.relu_mask_(ops.conv2d_k4s2(g3, PT['w4'], None, relu=False), a2)
+        dw2 = ops.conv_k4s2_wgrad(a1, g2)
+        db2 = _bias_grad(g2.view(-1, ch))
+        g1 = ops.relu_mask_(ops.conv2d_k4s2(g2, PT['w2'], None, relu=False), a1)
+        dw0 = ops.conv_k4s2_wgrad(x0, g1)
+        db0 = _bias_grad(g1.view(-1, ch))
+        dq = None
+        if ctx.needs_input_grad[0]:
+            dq = ops.conv2d_k4s2(g1, PT['w0'], None, relu=False).float()
+        return (dq, None, dw0, db0, dw2, db2, dw4, db4, dw6.view(3, ch, 1, 1), db6)
 
 
 class VQVAE(nn.Module):

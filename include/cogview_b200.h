@@ -395,6 +395,31 @@ int cv_vq_lookup(const int64_t* idx, const float* codebook, void* out_bf16, floa
 int cv_conv1x1_out3(const void* x, const float* w, const float* bias, const float* scale, const float* shift,
                     float* out, int B, int H, int W, int cin, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * VQ-VAE training (vqvae_zc.py in train() mode).  Every reduction runs in a fixed order: equal inputs, equal bits.
+ *   cv_conv_k4s2_wgrad: weight gradient of a k4 s2 p1 Conv2d or ConvTranspose2d.  With the small map
+ *     S [B, h, w, M] and the big map G [B, 2h, 2w, N] (NHWC bf16),
+ *       out[m, n, ky, kx] = sum_{b,y,x} S[b, y, x, m] * G[b, 2y - 1 + ky, 2x - 1 + kx, n]   (zero outside G), fp32.
+ *     Conv2d: S = dY, G = X -> dW [Cout, Cin, 4, 4].  ConvTranspose2d: S = X, G = dY -> dW [Cin, Cout, 4, 4].
+ *     M % 128 == 0, N % 256 == 0; workspace of cv_conv_k4s2_wgrad_workspace_bytes (split-K partials).
+ *   cv_relu_mask_bf16: dx[i] = act[i] > 0 ? dx[i] : 0 in place (act = the saved ReLU output); n % 8 == 0.
+ *   cv_conv1x1_out3_bwd: backward of the Decoder's last 1x1 conv (:191) from dr = dL/d(out) [B, 3, H, W] fp32 and
+ *     the saved ReLU output x [B, H, W, cin] bf16: dx = (dr . w) * (x > 0) bf16 NHWC, dw [3, cin] and db [3] fp32.
+ *     cin = 8 x a divisor of 256; workspace of cv_conv1x1_out3_bwd_workspace_bytes.
+ *   cv_vq_ema_stats: embed_onehot_sum (counts [n_embed]) and embed_sum = flatten^T . onehot ([dim, n_embed]) of
+ *     Quantize.forward_ (:68-69) from the codes idx [rows] and z [rows, dim] fp32; each code's rows are summed in
+ *     row order.
+ * ---------------------------------------------------------------------------------------------- */
+int64_t cv_conv_k4s2_wgrad_workspace_bytes(int B, int h, int w, int M, int N);
+int cv_conv_k4s2_wgrad(const void* S, const void* G, float* out, float* workspace, int B, int h, int w, int M, int N,
+                       void* stream);
+int cv_relu_mask_bf16(void* dx, const void* act, int64_t n, void* stream);
+int64_t cv_conv1x1_out3_bwd_workspace_bytes(int cin);
+int cv_conv1x1_out3_bwd(const float* dr, const void* x, const float* w, void* dx, float* dw, float* db,
+                        float* workspace, int B, int H, int W, int cin, void* stream);
+int cv_vq_ema_stats(const int64_t* idx, const float* z, int64_t rows, int dim, int n_embed, float* counts,
+                    float* embed_sum, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
