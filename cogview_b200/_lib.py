@@ -58,6 +58,7 @@ def _declare(lib):
         "cv_attn_decode": [P, P, L, P, I, P, P, I, I, I, I, I, P],
         "cv_attn_decode_ragged": [P, P, L, P, I, P, P, P, I, I, I, I, I, P],
         "cv_attn_chunk_ragged": [P, P, L, I, P, P, P, I, I, I, I, I, I, P],
+        "cv_attn_decode_shared": [P, P, L, I, I, P, L, P, I, I, P, P, I, I, I, I, I, P],
         "cv_sparse_plan": [P, L, P, I, I, I, I, I, P, P, I, P, P, P],
         "cv_attn_decode_gather": [P, P, L, P, P, L, P, P, P, I, I, I, I, I, P],
         "cv_adamw_step": [P, P, P, P, P, L, F, F, F, F, F, I, P, F, P],
@@ -108,6 +109,8 @@ def _declare(lib):
     lib.cv_attn_decode_workspace_bytes.restype = L
     lib.cv_attn_chunk_workspace_bytes.argtypes = [I, I, I, I]
     lib.cv_attn_chunk_workspace_bytes.restype = L
+    lib.cv_attn_shared_workspace_bytes.argtypes = [I, I, I]
+    lib.cv_attn_shared_workspace_bytes.restype = L
     lib.cv_launch_count.restype = ctypes.c_longlong
     lib.cv_set_reserved_sms.argtypes = [I]
     lib.cv_set_reserved_sms.restype = I

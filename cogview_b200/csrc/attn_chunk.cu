@@ -16,6 +16,7 @@
 // rather than a 64-row wgmma tile, and the K / V operands come straight from the XOR-swizzled tiles through
 // ldmatrix (.trans for V).  The MMAs are far from the bound either way; what matters is the single pass over the cache.
 #include "common.cuh"
+#include "mma_tile.cuh"
 #include "host.h"
 #include "../../include/cogview_b200.h"
 
@@ -39,31 +40,6 @@ struct ChunkParams {
     int n, heads, nsplit;
     float scale_log2;
 };
-
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool valid) {
-    const int sz = valid ? 16 : 0;                         // 0: zero-fill the 16 bytes
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(sz) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void cp_async_wait1() { asm volatile("cp.async.wait_group 1;" ::: "memory"); }
-
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
-                 : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
-                 : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
-// byte offset of 16-byte chunk c (8 head dims) of row r in a [rows][64] bf16 tile; the XOR swizzle puts the 8 rows
-// that one ldmatrix phase reads on 8 different bank groups
-__device__ __forceinline__ uint32_t swz(int r, int c) { return (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4)); }
 
 __global__ void __launch_bounds__(CK_THREADS)
 attn_chunk_kernel(const ChunkParams p) {

@@ -6,8 +6,8 @@ import torch
 
 from . import vqvae
 from .generation.magnify import magnify, magnify_batch
-from .generation.sampling import (add_interlacing_beam_marks, filling_sequence, filling_sequences, get_tokenizer,
-                                  inverse_prompt_score)
+from .generation.sampling import (add_interlacing_beam_marks, filling_sequence, filling_sequences,
+                                  filling_shared_prompts, get_tokenizer, inverse_prompt_score)
 
 # generate_samples.py:203-214
 QUERY_TEMPLATES = {
@@ -135,6 +135,51 @@ def generate_images_batch(model, vq_model, args, seqs, num=8, fill=filling_seque
                 group.append(seq)
             for rows in fill(model, group, args):
                 out.append((rows, _decode_rows(rows, decode)))
+    return out
+
+
+def caption_ids(row, tokenizer=None):
+    """The text ids after the last [ROI1] of a token row, un-offset as split_tokens gives them (what sentencepiece
+    decodes)."""
+    parts, _ = split_tokens(row.tolist() if torch.is_tensor(row) else row, tokenizer)
+    idx = max(i for i, p in enumerate(parts) if p == '[ROI1]')
+    return [x for p in parts[idx + 1:] if isinstance(p, list) for x in p]
+
+
+def image2text(model, vq_model, args, images, num=8, fill=filling_shared_prompts, encode=None):
+    """generate_samples.py:143-186, 202-221 for the 'image2text' task: `num` captions of every image.  images:
+    [N, 3, 256, 256], normalised as vqvae.img2code takes them (the reference's read_img: Resize and CenterCrop 256,
+    ToTensor, Normalize(IMG_MEAN, IMG_STD)).  The images are encoded (`encode`, default vqvae.img2code), each image's
+    query is QUERY_TEMPLATES['image2text'] ([BASE] [BOI1] codes [EOI1] [ROI1] [MASK]*20) with beams marked as the
+    reference marks them, nb = min(num, args.max_inference_batch_size), and whole images are packed into batches of at
+    most args.max_inference_batch_size rows.  `fill` takes a list of templates and returns a list of token tensors:
+    filling_shared_prompts reads each image's prompt K|V once for all of its beams, and falls back to
+    filling_sequences where it does not apply.  Returns one (token rows [num, 1048], captions) pair per image; captions
+    holds num lists of text ids (caption_ids: un-offset, for sentencepiece, which stays with the caller)."""
+    encode = encode or (lambda imgs: vqvae.img2code(vq_model, imgs))
+    tok = get_tokenizer(args)
+    mbz = args.max_inference_batch_size
+    assert num < mbz or num % mbz == 0
+    nb = min(num, mbz)
+    per_batch = max(1, mbz // nb)
+    model.eval()
+    with torch.no_grad():
+        codes = encode(images)
+        seqs = []
+        for c in codes:
+            seq = torch.tensor(build_query(QUERY_TEMPLATES['image2text'], [c.tolist()], tok), dtype=torch.long,
+                               device=codes.device)
+            add_interlacing_beam_marks(seq, nb=nb)
+            seqs.append(seq)
+        rows = [[] for _ in seqs]
+        for g0 in range(0, len(seqs), per_batch):
+            for _ in range(max(num // mbz, 1)):
+                for i, r in enumerate(fill(model, [seq.clone() for seq in seqs[g0:g0 + per_batch]], args)):
+                    rows[g0 + i].append(r)
+    out = []
+    for r in rows:
+        r = torch.cat(r, dim=0)
+        out.append((r, [caption_ids(row, tok) for row in r]))
     return out
 
 

@@ -494,6 +494,47 @@ def filling_sequences(model, seqs, args):
     return out
 
 
+def _shared_plan(model, tmpls, args, tokenizer):
+    """_batch_plan, and whether filling_shared_prompts can run the templates: _batch_plan's conditions (for one
+    template too), every context of the same length, and a model with shared_run."""
+    plans, ok = _batch_plan(model, tmpls, args, tokenizer)
+    return plans, ok and len({p[0] for p in plans}) == 1 and hasattr(model, 'shared_run')
+
+
+def filling_shared_prompts(model, seqs, args):
+    """filling_sequences for templates whose prompts are long next to what is generated (image2text: a 1028-token
+    image prompt, 20 text slots): returns one token tensor [nb, len(seq_c)] per template.  All contexts go through ONE
+    GPT2Model.forward at batch len(seqs) (logits of the last position only), whose K|V cache is the prefix every beam of
+    a template reads; the nb first tokens of each template are drawn from its prompt's logits as filling_sequence draws
+    them; the remaining slots run as one graph-replayed decode batch in which each prompt's K|V is read once for all of
+    its beams (GPT2Model.shared_run, cv_attn_decode_shared).  Needs the conditions of _batch_plan and contexts of one
+    length (_shared_plan); otherwise the templates go to filling_sequences.  The abs-max LayerNorm scales of the
+    prompt forward and of the decode step are taken over the whole batch, so a template's rows match a run of that
+    template alone within bf16 tolerance, not bit for bit."""
+    tokenizer = get_tokenizer(args)
+    tmpls = [seq.tolist() for seq in seqs]
+    plans, ok = _shared_plan(model, tmpls, args, tokenizer)
+    if not ok:
+        return filling_sequences(model, seqs, args)
+    device = seqs[0].device
+    C, offset, nb, n_gen = plans[0]
+    _, _, invalid_slices = _scan_context(tmpls[0], tokenizer)     # shared by all templates (_batch_plan)
+    tokens = torch.stack([seq[:C] for seq in seqs]).to(device)
+    attention_mask, _, position_ids = get_masks_and_position_ids(tokens)
+    position_ids = position_ids.clone()
+    position_ids[position_ids > offset] -= offset
+    logits, *mems = model(tokens, position_ids, attention_mask, None, None, 0, logits_last_only=True)
+    probs = _next_token_probs(logits, invalid_slices, args)
+    prev = torch.multinomial(probs, num_samples=nb, replacement=True)          # [templates, nb]
+    res = model.shared_run(prev.reshape(-1, 1), C - offset if C > offset else C, mems, n_gen - 1, args.temperature,
+                           args.top_k, invalid_slices)
+    if res is None:
+        raise RuntimeError('filling_shared_prompts: the decode batch of %d rows was refused' % prev.numel())
+    new_tokens = res[0].to(device)
+    return [torch.cat((tokens[i].expand(nb, -1), prev[i].view(nb, 1), new_tokens[i * nb:(i + 1) * nb]), dim=1)
+            for i in range(len(seqs))]
+
+
 def inverse_prompt_score(model, seq, args):
     """generation/sampling.py:214-230 — caption log-likelihood given the image (post-selection)."""
     tokenizer = get_tokenizer(args)

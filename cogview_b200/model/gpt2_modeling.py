@@ -178,6 +178,41 @@ def _generate_run_impl(self, last_tokens, first_pos, mems, n_steps, temperature,
 GPT2Model.generate_run = _generate_run_impl
 
 
+def _shared_run_impl(self, last_tokens, first_pos, mems, n_steps, temperature, top_k, invalid_slices):
+    """generate_run for rows that share prompts: `mems` are the K|V-cache views GPT2Model.forward returned for
+    `groups` prompts of one length P (the pooled cache of batch size groups), and the b rows of last_tokens [b, 1]
+    (b a multiple of groups) are their beams, G = b / groups consecutive rows per prompt, all at position first_pos.
+    Each prompt's K|V stays once in that cache and is read by cv_attn_decode_shared for all of its beams
+    (DecodeRunner's shared mode); the rows' own tokens go to a suffix cache of n_steps slots (kv_cache.shared).
+    Returns None when the fast path does not apply, else (tokens [b, n_steps], summed log-probabilities [b])."""
+    tr = self.transformer
+    b = last_tokens.shape[0]
+    if (not mems or tr.mems_mode != 'kv' or tr.max_memory_length <= 0 or torch.is_grad_enabled()
+            or not ops.decode_batch_supported(b, tr.hidden_size) or n_steps < 1
+            or os.environ.get('COGVIEW_B200_FAST_DECODE', '1') == '0'
+            or os.environ.get('COGVIEW_B200_GRAPH_SAMPLING', '1') == '0'):
+        return None
+    from ..mpu import kv_cache
+    from ..mpu.decode import DecodeRunner
+    groups, P = mems[0].size(0), mems[0].size(1)
+    prefix = tr.__dict__.get('_kv_pool', {}).get(groups)
+    if b % groups != 0 or b // groups > 64 or P < 1 or prefix is None or not prefix.matches(mems, groups):
+        return None
+    caches = kv_cache.shared(tr, prefix, P, b, n_steps)
+    try:
+        runner = caches.runner
+        if runner is None:
+            runner = caches.runner = DecodeRunner(self, caches,
+                                                  use_graph=os.environ.get('COGVIEW_B200_CUDA_GRAPH', '1') != '0')
+        pos = torch.full((b, 1), int(first_pos), dtype=torch.long, device=last_tokens.device)
+        return runner.sample_run(last_tokens.reshape(b, 1), pos, 0, n_steps, temperature, top_k, invalid_slices)
+    finally:
+        caches.prefix = None
+
+
+GPT2Model.shared_run = _shared_run_impl
+
+
 def _chunk_run_impl(self, tokens, position_ids, mems, row_pad=None):
     """n given tokens per row on the K|V cache in one eager pass — the model call generation/sampling.py:147-151
     makes for a template stretch of provided tokens (plus the last sampled one), for a batch whose rows sit at

@@ -7,7 +7,10 @@ Two device paths:
   * default: one kernel per operation (cv_attn_decode between cv_linear_small_m / cv_ln_pair_small_m at batch <= 16,
     cv_linear_mid_m / cv_ln_pair_mid_m at batch 17..64), CUDA-graph captured; in generation runs followed by ONE
     sampling kernel (cv_sample_topk) inside the same graph.  In ragged mode (rows from prompts of different lengths,
-    row_pad given) the attention is cv_attn_decode_ragged: row i holds cur_len - row_pad[i] cached tokens.
+    row_pad given) the attention is cv_attn_decode_ragged: row i holds cur_len - row_pad[i] cached tokens.  In shared
+    mode (a runner built on a kv_cache._SharedCaches: the beams of several prompts, each prompt's K|V held once) the
+    attention is cv_attn_decode_shared over the prompts' prefix cache and the rows' own suffix cache, and cur_len is
+    the suffix length.
   * COGVIEW_B200_PERSISTENT=1 and batch <= 8: the whole step — embedding, 48 Sandwich-LN layers, final LayerNorm,
     logits — is ONE persistent kernel (cv_decode_step, csrc/decode_step.cu: bulk-copy weight stream through a
     shared-memory byte ring, register-resident residual stream, grid barriers between the dependency points).  Parity-
@@ -42,15 +45,17 @@ class DecodeRunner:
         # ragged mode: row i holds cur_len - row_pad[i] cached tokens; captured graphs read this static buffer
         self.ragged = False
         self.row_pad = torch.zeros(self.b, dtype=torch.int32, device=dev)
-        self.step_graphs = {}            # ragged (bool) -> captured step
+        self.step_graphs = {}            # ragged (bool), or the prefix in shared mode -> captured step
         self.use_graph = use_graph
+        # shared mode: caches is a kv_cache._SharedCaches (suffix cache of b rows over the prefix cache of its groups)
+        self.shared = hasattr(caches, 'groups')
         assert self.b <= ops.DECODE_MAX_BATCH
         # which pair of kernels runs the linears and the Sandwich-LN glue is a property of the batch size
         small = self.b <= ops.DECODE_SMALL_MAX_BATCH
         self.linear = ops.linear_small_m if small else ops.linear_mid_m
         self.ln_pair = ops.ln_pair_small_m if small else ops.ln_pair_mid_m
         self.persistent = (_persistent_enabled() and self.b <= ops.DECODE_STEP_MAX_BATCH and self.h % 256 == 0
-                           and self.h <= 2560)
+                           and self.h <= 2560 and not self.shared)
         # enough (batch, head, split) CTAs to cover the SMs
         sms = torch.cuda.get_device_properties(dev).multi_processor_count
         # the key range of every (batch, head) is split so that ~8 CTAs per SM stream the K|V cache: the kernel is
@@ -135,6 +140,8 @@ class DecodeRunner:
             self.is_txt.scatter_(1, self.len64.expand(b, 1), (self.ids >= sparse['n_img']).to(torch.uint8))
             ops.sparse_plan(self.is_txt, self.cur_len, L, self.window, tr.num_pivot, tr.max_sequence_length, self.seed_dev,
                             self.key_idx, self.n_keys, self.plan_err)
+        if self.shared:
+            shared_nsplit = ops.attn_chunk_nsplit(self.caches.groups, heads, self.caches.P, self.ids.device)
         x = ops.embed_fwd(self.ids, self.pos, self.wte, self.wpe, scal[2 * L:2 * L + 1])
         prev_gemm = prev_am = prev_post = None
         for i, P in enumerate(self.params):
@@ -146,7 +153,10 @@ class DecodeRunner:
             if y is not None:
                 x = y
             qkv = self.linear(xn, wqkv, bqkv)
-            if sparse is not None:
+            if self.shared:
+                ctx = ops.attn_decode_shared(qkv, self.caches.prefix.buf[i], self.caches.buf[i], heads, self.caches.P,
+                                             s_dev=self.cur_len, nsplit=shared_nsplit)
+            elif sparse is not None:
                 ctx = ops.attn_decode_gather(qkv, self.caches.buf[i], heads, self.cur_len, self.key_idx[i], self.n_keys,
                                              nsplit=self.nsplit)
             else:
@@ -166,14 +176,23 @@ class DecodeRunner:
 
     def _set_rows(self, row_pad):
         """Uniform (row_pad None) or ragged mode for the next step or run."""
+        assert not (self.shared and row_pad is not None)
         self.ragged = row_pad is not None
         if self.ragged:
             assert row_pad.shape == (self.b,)
             self.row_pad.copy_(row_pad)
 
+    def _mode(self):
+        """Key of the captured graphs: ragged or not, or in shared mode the prefix cache the graphs read (its buffer,
+        stride and length are baked into them)."""
+        if self.shared:
+            pre = self.caches.prefix.buf
+            return ('shared', pre.data_ptr(), pre.stride(1), self.caches.P)
+        return self.ragged
+
     def step(self, ids, pos, t, row_pad=None):
         """ids, pos: [b, 1] int64; t: tokens already cached (in ragged mode, in the longest row; row i holds
-        t - row_pad[i]).  Returns logits [b, V] fp32 (a static buffer that the next step overwrites; the sampling
+        t - row_pad[i]; in shared mode, in every row's suffix).  Returns logits [b, V] fp32 (a static buffer that the next step overwrites; the sampling
         graphs never modify it)."""
         if self.params is None or t <= self.last_t:      # a new sequence: make sure the weights are the live ones
             self._check_params()
@@ -182,7 +201,7 @@ class DecodeRunner:
         self.ids.copy_(ids)
         self.pos.copy_(pos)
         self.cur_len.fill_(t)
-        graph = self.step_graphs.get(self.ragged)
+        graph = self.step_graphs.get(self._mode())
         if not self.use_graph:
             self._run()
         elif graph is None:
@@ -194,7 +213,7 @@ class DecodeRunner:
             torch.cuda.current_stream().wait_stream(side)
             from .._lib import lib
             before = lib().cv_launch_count()
-            graph = self.step_graphs[self.ragged] = torch.cuda.CUDAGraph()
+            graph = self.step_graphs[self._mode()] = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
                 self._run()
             self.graph_launches = int(lib().cv_launch_count() - before)
@@ -257,13 +276,16 @@ class DecodeRunner:
         token.  Returns (tokens [b, n_steps] int64, summed log-probabilities [b] fp32).
         sparse: None, or dict(n_img=..., tokens=[b, t + 1] every token so far) for is_sparse == 2.
         row_pad: None, or int32 [b] on the device: row i holds t - row_pad[i] cached tokens (ragged mode; not with
-        sparse)."""
+        sparse).  In shared mode t is the suffix length and t + n_steps must fit the suffix cache."""
         assert sparse is None or row_pad is None
+        assert not self.shared or (sparse is None and t + n_steps <= self.caches.maxlen)
         self._check_params()
         self.last_t = t + n_steps
         vocab = self.model.word_embeddings.weight.shape[0]
         key = (float(temperature), int(top_k), tuple(sl.indices(vocab)[:2] for sl in invalid_slices),
                None if sparse is None else int(sparse['n_img']), row_pad is not None)
+        if self.shared:
+            key += (self._mode(),)
         assert n_steps <= self.out_buf.shape[1]
         self._set_rows(row_pad)
         self.sparse = None

@@ -71,12 +71,13 @@ def cache_bytes(owner, b):
     return len(owner.layers) * b * owner.max_memory_length * 2 * owner.hidden_size * 2
 
 
-def _make_room(owner, pool, b):
-    """Called before a cache for batch size b is allocated: drop pooled caches of other sizes, largest first, until
-    the pool with the new cache fits POOL_BYTE_BUDGET (the new cache itself is always allowed)."""
-    need = cache_bytes(owner, b)
-    others = sorted((k for k in pool if k != b), key=lambda k: pool[k].buf.numel(), reverse=True)
-    total = need + sum(pool[k].buf.numel() * 2 for k in others)
+def _make_room(owner, pool, b, need=None, keep=()):
+    """Called before a cache for batch size b (or pool key b) is allocated: drop pooled caches of other sizes, largest
+    first, until the pool with the new cache of `need` bytes (default: cache_bytes) fits POOL_BYTE_BUDGET (the new
+    cache itself is always allowed).  The keys in `keep` are counted but not dropped."""
+    need = cache_bytes(owner, b) if need is None else need
+    total = need + sum(pool[k].buf.numel() * 2 for k in pool if k != b)
+    others = sorted((k for k in pool if k != b and k not in keep), key=lambda k: pool[k].buf.numel(), reverse=True)
     for k in others:
         if total <= POOL_BYTE_BUDGET:
             break
@@ -179,3 +180,39 @@ def assemble_rows(owner, lens, rows, run, prefill):
     row_pad = torch.tensor([t - ln for ln, n in zip(lens, rows) for _ in range(n)], dtype=torch.int32,
                            device=c.buf.device)
     return [c.buf[i, :, :t] for i in range(c.L)] + [c.dummy[:, :t]], row_pad
+
+
+class _SharedCaches:
+    """The generated tokens of a decode batch whose rows share prompts (DecodeRunner's shared mode): b rows in `groups`
+    groups of G = b / groups consecutive rows.  Group g's prompt K|V is row g of the pooled cache of batch size groups
+    (`prefix`, P tokens, filled by one forward over the prompts and only read by the decode); row r's generated
+    tokens go to buf[:, r, :maxlen]."""
+
+    def __init__(self, owner, b, groups, run, device):
+        self.h = owner.hidden_size
+        self.L = len(owner.layers)
+        self.b, self.groups, self.maxlen = b, groups, run
+        self.buf = torch.empty((self.L, b, run, 2 * self.h), dtype=torch.bfloat16, device=device)
+        self.prefix, self.P = None, 0
+        self.runner = None
+
+
+def shared(owner, prefix, P, b, run):
+    """The suffix cache of b rows continuing the prefix.b prompts of the pooled cache `prefix` (P tokens each), with room
+    for `run` tokens per row.  It is pooled under ('shared', b, groups, run) with its DecodeRunner, so the next batch of
+    the same shape reuses both, and its bytes count against POOL_BYTE_BUDGET; the prefix cache is never dropped to
+    make room for it.  The caller sets .prefix back to None after the run, so that the suffix cache does not keep a
+    prefix cache alive that the pool has since dropped."""
+    assert b % prefix.b == 0 and 0 < P and P <= prefix.maxlen and run >= 1
+    pool = owner.__dict__.setdefault('_kv_pool', {})
+    assert pool.get(prefix.b) is prefix
+    key = ('shared', b, prefix.b, run)
+    c = pool.get(key)
+    if c is not None and c.buf.device != prefix.buf.device:
+        c = None
+        del pool[key]
+    if c is None:
+        _make_room(owner, pool, key, need=len(owner.layers) * b * run * 2 * owner.hidden_size * 2, keep=(prefix.b,))
+        c = pool[key] = _SharedCaches(owner, b, prefix.b, run, prefix.buf.device)
+    c.prefix, c.P = prefix, P
+    return c

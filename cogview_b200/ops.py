@@ -389,6 +389,36 @@ def attn_chunk_ragged(qkv, cache, heads, cur_len, row_pad=None, *, nsplit=None, 
     return out
 
 
+def attn_decode_shared(qkv, prefix, suffix, heads, prefix_len, *, s=None, s_dev=None, nsplit=None, out=None,
+                       workspace=None):
+    """Decode attention for rows that share a prompt (cv_attn_decode_shared).  qkv: [b, 3h] bf16; prefix:
+    [groups, max_len, 2h] bf16 (K|V of every group's prompt, prefix_len tokens each; read only); suffix:
+    [b, s_max, 2h] bf16 (K|V of every row's generated tokens).  Row r of group r // (b // groups) attends
+    prefix[g, :prefix_len], suffix[r, :s] and its new key, and its k|v is written at suffix[r, s].  s from the host,
+    or from s_dev (int32 [1] on the device, read when the kernel runs).  Returns the context [b, h] bf16."""
+    require_cuda(qkv, prefix, suffix, s_dev)
+    b, h3 = qkv.shape
+    h = h3 // 3
+    groups = prefix.shape[0]
+    assert qkv.dtype == prefix.dtype == suffix.dtype == torch.bfloat16 and qkv.is_contiguous()
+    for c in (prefix, suffix):
+        assert c.stride(2) == 1 and c.stride(1) == 2 * h and c.shape[2] == 2 * h
+    assert suffix.shape[0] == b and (s_dev is None or s_dev.dtype == torch.int32)
+    if nsplit is None:
+        nsplit = attn_chunk_nsplit(groups, heads, prefix_len, qkv.device)
+    if out is None:
+        out = torch.empty((b, h), dtype=torch.bfloat16, device=qkv.device)
+    if workspace is None:
+        workspace = torch.empty(lib().cv_attn_shared_workspace_bytes(b, heads, nsplit) // 4, dtype=torch.float32,
+                                device=qkv.device)
+    rc = lib().cv_attn_decode_shared(ptr(qkv), ptr(prefix), prefix.stride(0), int(prefix_len), prefix.shape[1],
+                                     ptr(suffix), suffix.stride(0), ptr(s_dev), -1 if s is None else int(s),
+                                     suffix.shape[1], ptr(out), ptr(workspace), b, groups, heads, 64, nsplit,
+                                     stream_ptr())
+    check(rc, "cv_attn_decode_shared")
+    return out
+
+
 def sparse_plan(is_txt, cur_len_dev, num_layers, window, num_pivot, max_sequence_length, seed_dev, idx, n_dev, err):
     """Index plan of one sparse decode step for every layer (cv_sparse_plan).  is_txt: uint8 [b, max_len]; idx: int32
     [num_layers, b, nmax] (written); n_dev, err: int32 [1]; seed_dev: int64 [1]."""

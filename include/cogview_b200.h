@@ -256,6 +256,24 @@ int64_t cv_attn_chunk_workspace_bytes(int b, int heads, int n, int nsplit);
 int cv_attn_chunk_ragged(const void* qkv, void* cache, int64_t cache_batch_stride, int cur_len, const int* row_pad,
                          void* out, float* workspace, int b, int n, int heads, int head_dim, int max_len, int nsplit,
                          void* stream);
+/* standard_attention (mpu/sparse_transformer.py:652-673) for sq = 1, as cv_attn_decode, for rows that share a prompt
+ * (csrc/attn_shared.cu): the beams of one image in image-to-text sampling (generate_samples.py:161-186).  The b rows
+ * form `groups` groups of G = b / groups consecutive rows; the prompt's K|V is held once per group.
+ * qkv [b, 3h] bf16: q | k_new | v_new of each row.  prefix [groups, max_len, 2h] bf16 (K | V, batch stride
+ * prefix_batch_stride elements), read only: every group's prompt is prefix_len = P tokens long.  suffix [b, s_max, 2h]
+ * bf16 (K | V, batch stride suffix_batch_stride): row r's generated tokens.  The suffix length s comes from *s_dev when
+ * non-NULL (so a captured CUDA graph can be replayed), else from s.  Row r of group g = r / G attends, in this order,
+ * to prefix[g, 0:P], suffix[r, 0:s] and its new key: softmax of the scores scaled by 1/sqrt(64).  Row r's k|v is
+ * written at suffix[r, s]; nothing else in either buffer is written.  out [b, h] bf16.  Every prefix key and value is
+ * read once per (group, head); nsplit (1..64) splits the prefix keys over that many CTAs, and a second kernel per
+ * (row, head) adds the suffix and the new key and merges.  workspace: cv_attn_shared_workspace_bytes(b, heads, nsplit)
+ * bytes, always required.  Argument errors: head_dim != 64, G outside 1..64 or b % groups != 0, P > max_len,
+ * s >= s_max (s from the host), nsplit outside 1..64, misaligned pointers.  Contract (not checked, device data):
+ * 0 <= *s_dev < s_max. */
+int64_t cv_attn_shared_workspace_bytes(int b, int heads, int nsplit);
+int cv_attn_decode_shared(const void* qkv, const void* prefix, int64_t prefix_batch_stride, int prefix_len, int max_len,
+                          void* suffix, int64_t suffix_batch_stride, const int* s_dev, int s, int s_max, void* out,
+                          float* workspace, int b, int groups, int heads, int head_dim, int nsplit, void* stream);
 /* Sparse inference (is_sparse == 2, mpu/sparse_transformer.py:498-520, :591-600, :727-750) without the host:
  *   cv_sparse_plan: the key index list of one decode step for EVERY layer: idx [num_layers, b, nmax] int32, *n_dev = its
  *     length.  Per (layer, sequence): every text position before the trailing window (is_txt [b, max_len] uint8 marks
