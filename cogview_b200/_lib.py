@@ -77,6 +77,9 @@ def _declare(lib):
         "cv_relu_mask_bf16": [P, P, L, P],
         "cv_conv1x1_out3_bwd": [P, P, P, P, P, P, P, I, I, I, I, P],
         "cv_vq_ema_stats": [P, P, L, I, I, P, P, P],
+        "cv_gumbel_noise": [U64, L, L, I, P, P],
+        "cv_vq_gumbel_fwd": [P, L, P, L, I, U64, L, F, P, I, L, P, P, P],
+        "cv_vq_gumbel_bwd": [P, L, P, L, I, U64, L, F, P, L, F, P, L, P, P],
         "cv_embed_fwd": [P, P, P, P, P, P, I, I, F, U64, U32, P],
         "cv_embed_bwd": [P, P, P, P, P, I, I, F, U64, U32, P],
         "cv_dropout_mask": [P, L, F, U64, U32, P],

@@ -688,6 +688,50 @@ def vq_ema_stats(idx, z, n_embed):
     return counts, embed_sum
 
 
+def gumbel_noise(seed, row0, rows, K, device="cuda"):
+    """The Gumbel(0, 1) noise [rows, K] fp32 of absolute rows row0 .. row0 + rows - 1 that vq_gumbel_fwd / _bwd use."""
+    out = torch.empty((rows, K), dtype=torch.float32, device=device)
+    check(lib().cv_gumbel_noise(int(seed), int(row0), rows, K, ptr(out), stream_ptr()), "cv_gumbel_noise")
+    return out
+
+
+def _check_scores(scores, e2):
+    require_cuda(scores, e2)
+    assert scores.dtype == torch.float32 and scores.dim() == 2 and scores.stride(1) == 1
+    assert e2.dtype == torch.float32 and e2.is_contiguous() and e2.numel() == scores.shape[1]
+
+
+def vq_gumbel_fwd(scores, e2, seed, row0, tau, *, y_dtype=torch.bfloat16, want_kl=False):
+    """Gumbel softmax over the codes, per row of scores [rows, K] fp32 (z.E) and e2 [K] (|e|^2).
+    Returns (y [rows, K] of y_dtype, or None when y_dtype is None; idx [rows] int64; kl [rows] fp32 or None)."""
+    _check_scores(scores, e2)
+    rows, K = scores.shape
+    y = None if y_dtype is None else torch.empty((rows, K), dtype=y_dtype, device=scores.device)
+    assert y_dtype in (None, torch.bfloat16, torch.float32)
+    idx = torch.empty(rows, dtype=torch.int64, device=scores.device)
+    kl = torch.empty(rows, dtype=torch.float32, device=scores.device) if want_kl else None
+    check(lib().cv_vq_gumbel_fwd(ptr(scores), scores.stride(0), ptr(e2), rows, K, int(seed), int(row0), float(tau),
+                                 ptr(y), int(y_dtype == torch.float32), K, ptr(idx), ptr(kl), stream_ptr()),
+          "cv_vq_gumbel_fwd")
+    return y, idx, kl
+
+
+def vq_gumbel_bwd(scores, e2, seed, row0, tau, dy=None, kl_scale=0.0):
+    """Backward of vq_gumbel_fwd's y (from dy [rows, K] fp32) and of its KL (scaled by kl_scale) to the logits
+    a = 2 scores - e2.  Returns (da [rows, K] bf16, rowsum [rows] fp32 = sum_j da)."""
+    _check_scores(scores, e2)
+    rows, K = scores.shape
+    if dy is not None:
+        require_cuda(dy)
+        assert dy.dtype == torch.float32 and dy.shape == (rows, K) and dy.stride(1) == 1
+    da = torch.empty((rows, K), dtype=torch.bfloat16, device=scores.device)
+    rowsum = torch.empty(rows, dtype=torch.float32, device=scores.device)
+    check(lib().cv_vq_gumbel_bwd(ptr(scores), scores.stride(0), ptr(e2), rows, K, int(seed), int(row0), float(tau),
+                                 ptr(dy), 0 if dy is None else dy.stride(0), float(kl_scale), ptr(da), K, ptr(rowsum),
+                                 stream_ptr()), "cv_vq_gumbel_bwd")
+    return da, rowsum
+
+
 def attn_gather(q, cache, idx, heads):
     """sparse_attention_inference: q [b, sq, h] view, cache [b, max_len, 2h] (K|V), idx [b, n] int64 -> [b, sq, h]."""
     require_cuda(q, cache, idx)

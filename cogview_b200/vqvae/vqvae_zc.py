@@ -3,8 +3,11 @@
 class names, constructor arguments, parameter/buffer names (state_dict keys `enc_b.blocks.{0,2,4,6}`,
 `quantize_t.{embed,cluster_size,embed_avg}`, `dec.blocks.{0,2,4,6}`) and method signatures, on the inference
 paths `encode` (img -> codes) and `decode_code` (codes -> img), and in train() mode `forward` (img -> recon, diff)
-with the EMA codebook update (vqvae_zc.py:67-83) and a backward for every parameter.  The gumbel relaxations
-(continuous_relax=True, :55-64, :87-91, :284-346) are not accelerated and raise.
+with the EMA codebook update (vqvae_zc.py:67-83) and a backward for every parameter.  The Gumbel-softmax
+relaxations (continuous_relax=True: soft :55-60, hard :61-65 with the EMA update, the KL :87-92, gumbel_softmax
+:284-346) run in train and eval mode, with `KL` passed through VQVAE.forward / encode.  Their noise is Gumbel(0, 1)
+from a counter-based Philox stream under one seed per call drawn from torch's default generator: the same
+distribution as the reference's torch.exponential_ draws, not the same numbers.
 
 Device layout: NHWC bf16 activations; the three stride-2 4x4 convolutions and the three transposed convolutions run
 as im2col-free wgmma implicit GEMMs (cv_conv2d_k4s2 / cv_conv_transpose2d_k4s2), the Cin=3 first conv as
@@ -12,7 +15,9 @@ im2col + GEMM, the 1x1 convs as GEMMs, the quantiser as a 3-term bf16-split tens
 Training: one autograd Function per network half (_EncoderFn, _DecoderFn) saves the bf16 ReLU outputs; data gradients
 run on the forward convolution kernels with the adjoint packing (the data gradient of Conv2d(k4, s2, p1) is
 ConvTranspose2d(k4, s2, p1) with the same weight, and the reverse) followed by the ReLU mask, weight gradients on
-cv_conv_k4s2_wgrad and the GEMM's wgrad operand modes, bias gradients on cv_colsum_bf16."""
+cv_conv_k4s2_wgrad and the GEMM's wgrad operand modes, bias gradients on cv_colsum_bf16.  Relaxed quantiser: the
+split3 score GEMM, then cv_vq_gumbel_fwd (noised tempered softmax y, arg-max, KL) and y @ E^T on the GEMM; its
+backward (_GumbelFn) recomputes the scores from the saved z and runs dq @ E, cv_vq_gumbel_bwd and da @ E^T."""
 import torch
 from torch import nn
 
@@ -70,9 +75,17 @@ class Quantize(nn.Module):
             return et, packed, e2
         return self._cache.get("tables", [self.embed], build)
 
-    def forward_(self, input, continuous_relax=False, temperature=1., hard=False):
+    def _gumbel_tables(self):
+        """bf16 codebook E [dim, n_embed] (the GEMM operand of y @ E^T and da @ E^T) and E^T [n_embed, dim] (dq @ E)."""
+        return self._cache.get("gumbel", [self.embed],
+                               lambda: (self.embed.detach().to(torch.bfloat16).contiguous(),
+                                        self.embed.detach().t().to(torch.bfloat16).contiguous()))
+
+    def forward_(self, input, continuous_relax=False, temperature=1., hard=False, kl=True):
+        """vqvae_zc.py:41-93.  `kl` (not in the reference) is False when the caller discards the KL, as VQVAE.encode
+        does without KL=True: diff is then the zero placeholder of :258 and the KL is not computed."""
         if continuous_relax:
-            raise NotImplementedError('only the hard nearest-code path is accelerated (continuous_relax=False)')
+            return self._forward_relaxed(input, temperature, hard, kl)
         if self.training:
             return self._forward_train(input)
         flatten = input.reshape(-1, self.dim).float().contiguous()
@@ -104,6 +117,13 @@ class Quantize(nn.Module):
         embed_ind, et = self._nearest(flatten)
         _, quant = ops.vq_lookup(embed_ind, et, want_bf16=False, want_f32=True)
         quant = quant.view(*input.shape)
+        self._ema_update(embed_ind, flatten)
+        diff = (quant - input).pow(2).mean()
+        quantize = input + (quant - input).detach()        # straight-through estimator
+        return quantize, diff, embed_ind.view(*input.shape[:-1])
+
+    def _ema_update(self, embed_ind, flatten):
+        """vqvae_zc.py:67-83 from the chosen codes and the fp32 rows they were chosen for."""
         embed_onehot_sum, embed_sum = ops.vq_ema_stats(embed_ind, flatten, self.n_embed)
         with torch.no_grad():
             self.cluster_size.mul_(self.decay).add_(embed_onehot_sum, alpha=1 - self.decay)
@@ -111,9 +131,21 @@ class Quantize(nn.Module):
             n = self.cluster_size.sum()
             cluster_size = (self.cluster_size + self.eps) / (n + self.n_embed * self.eps) * n
             self.embed.copy_(self.embed_avg / cluster_size.unsqueeze(0))
-        diff = (quant - input).pow(2).mean()
-        quantize = input + (quant - input).detach()        # straight-through estimator
-        return quantize, diff, embed_ind.view(*input.shape[:-1])
+
+    def _forward_relaxed(self, input, temperature, hard, kl):
+        """vqvae_zc.py:55-65, :67-83 (hard only, in train() mode), :87-92.  The noise comes from the kernels' counter
+        stream under one seed drawn from torch's default generator per call (torch.manual_seed repeats a run)."""
+        _check_temperature(temperature)
+        seed = int(torch.randint(0, 2 ** 62, (1,), dtype=torch.int64).item())
+        flatten = input.reshape(-1, self.dim)
+        if hard and not kl:        # nothing differentiable leaves: the lookup carries no gradient (:65)
+            quant, _, embed_ind = _gumbel_forward(flatten.detach().float().contiguous(), self, seed, float(temperature), True, False)
+            diff = torch.zeros((), dtype=torch.float32, device=input.device)
+        else:
+            quant, diff, embed_ind = _GumbelFn.apply(flatten, self, seed, float(temperature), hard, kl)
+        if self.training and hard:
+            self._ema_update(embed_ind, flatten.detach().float().contiguous())
+        return quant.view(*input.shape), diff, embed_ind.view(*input.shape[:-1])
 
     def embed_code(self, embed_id):
         et, _, _ = self._tables()
@@ -311,6 +343,87 @@ class _DecoderFn(torch.autograd.Function):
         return (dq, None, dw0, db0, dw2, db2, dw4, db4, dw6.view(3, ch, 1, 1), db6)
 
 
+def _check_temperature(temperature):
+    # the reference divides by it unchecked and returns inf or NaN for tau <= 0
+    if not temperature > 0:
+        raise ValueError('the Gumbel-softmax temperature must be positive, got %r' % (temperature,))
+
+
+def _gumbel_forward(z, q, seed, tau, hard, kl):
+    """The relaxed quantiser on fp32 rows z [rows, dim], score_chunk_rows rows at a time: the split3 score GEMM, then
+    cv_vq_gumbel_fwd.  Soft: quant = y @ E^T (bf16 y, bf16 E, fp32 accumulation).  Hard: quant = the code's row of
+    the current codebook.  Returns (quant [rows, dim] fp32, the KL mean (or None), idx [rows])."""
+    et, packed, e2 = q._tables()
+    e_bf, _ = q._gumbel_tables()
+    rows = z.shape[0]
+    quant = None if hard else torch.empty((rows, q.dim), dtype=torch.float32, device=z.device)
+    idx, kls = [], []
+    for r0 in range(0, rows, q.score_chunk_rows):
+        zc = z[r0:r0 + q.score_chunk_rows]
+        scores = ops.gemm(ops.vq_split3(zc), packed, out_dtype=torch.float32)
+        y, i, k = ops.vq_gumbel_fwd(scores, e2, seed, r0, tau, y_dtype=None if hard else torch.bfloat16, want_kl=kl)
+        del scores
+        if not hard:
+            ops.gemm(y, e_bf, out_dtype=torch.float32, out=quant[r0:r0 + zc.shape[0]])
+        idx.append(i)
+        kls.append(k)
+    idx = torch.cat(idx)
+    if hard:
+        _, quant = ops.vq_lookup(idx, et, want_bf16=False, want_f32=True)
+    return quant, (torch.cat(kls).mean() if kl else None), idx
+
+
+class _GumbelFn(torch.autograd.Function):
+    """The relaxed quantiser of Quantize.forward_ (vqvae_zc.py:55-65, :89-90) and its backward to z.  Saved: z and
+    the seed; the scores, y and qy are recomputed in the backward, score_chunk_rows rows at a time.
+
+    Backward, as the reference's autograd computes it: with a = -dist, dL/da from cv_vq_gumbel_bwd (the y term from
+    dy = dq @ E in soft mode, the KL term when the KL is in the loss), then dz = 2 da @ E^T - 2 z rowsum(da).  The
+    scores are those of the forward's codebook; the two GEMMs with E read the codebook as it is at backward time,
+    because the reference's matmul backward reads the buffer, which its hard-mode EMA update rewrites through .data
+    in between (:83)."""
+
+    @staticmethod
+    def forward(ctx, z, q, seed, tau, hard, kl):
+        zd = z.detach().float().contiguous()
+        quant, diff, idx = _gumbel_forward(zd, q, seed, tau, hard, kl)
+        if diff is None:
+            diff = torch.zeros((), dtype=torch.float32, device=z.device)
+            ctx.mark_non_differentiable(diff)
+        if hard:
+            ctx.mark_non_differentiable(quant)
+        ctx.mark_non_differentiable(idx)
+        ctx.save_for_backward(zd)
+        _, packed, e2 = q._tables()
+        ctx.scores_tables = (packed, e2)
+        ctx.q, ctx.seed, ctx.tau, ctx.hard, ctx.kl = q, seed, tau, hard, kl
+        return quant, diff, idx
+
+    @staticmethod
+    def backward(ctx, dq, ddiff, _didx):
+        (z,) = ctx.saved_tensors
+        q = ctx.q
+        rows = z.shape[0]
+        want_y = not ctx.hard and dq is not None
+        kl_scale = float(ddiff) / rows if (ctx.kl and ddiff is not None) else 0.0
+        if not want_y and kl_scale == 0.0:
+            return None, None, None, None, None, None
+        packed, e2 = ctx.scores_tables
+        e_bf, et_bf = q._gumbel_tables()
+        dqb = dq.reshape(rows, q.dim).to(torch.bfloat16).contiguous() if want_y else None
+        dz = torch.empty_like(z)
+        for r0 in range(0, rows, q.score_chunk_rows):
+            zc = z[r0:r0 + q.score_chunk_rows]
+            r1 = r0 + zc.shape[0]
+            scores = ops.gemm(ops.vq_split3(zc), packed, out_dtype=torch.float32)
+            dy = ops.gemm(dqb[r0:r1], et_bf, out_dtype=torch.float32) if want_y else None
+            da, rowsum = ops.vq_gumbel_bwd(scores, e2, ctx.seed, r0, ctx.tau, dy, kl_scale)
+            del scores, dy
+            g = ops.gemm(da, e_bf, out_dtype=torch.float32)                   # da @ E^T
+            dz[r0:r1] = 2.0 * (g - zc * rowsum.unsqueeze(1))
+        return dz, None, None, None, None, None
+
+
 class VQVAE(nn.Module):
     """vqvae_zc.py:217-269."""
 
@@ -329,8 +442,14 @@ class VQVAE(nn.Module):
         return self.dec(quant_t), diff
 
     def encode(self, input, continuous_relax=False, temperature=1., hard=False, KL=False):
+        if not continuous_relax:
+            logits = self.enc_b(input)
+            quant_t, diff_t, id_t = self.quantize_t.forward_(logits, continuous_relax, temperature, hard)
+            return quant_t.permute(0, 3, 1, 2), diff_t.unsqueeze(0), id_t
+        _check_temperature(temperature)
         logits = self.enc_b(input)
-        quant_t, diff_t, id_t = self.quantize_t.forward_(logits, continuous_relax, temperature, hard)
+        # without KL the reference returns zeros_like(diff) (:255-258); the KL is then not computed
+        quant_t, diff_t, id_t = self.quantize_t.forward_(logits, True, temperature, hard, kl=KL)
         return quant_t.permute(0, 3, 1, 2), diff_t.unsqueeze(0), id_t
 
     def decode(self, code):

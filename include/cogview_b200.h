@@ -438,6 +438,31 @@ int cv_conv1x1_out3_bwd(const float* dr, const void* x, const float* w, void* dx
 int cv_vq_ema_stats(const int64_t* idx, const float* z, int64_t rows, int dim, int n_embed, float* counts,
                     float* embed_sum, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Gumbel-softmax quantiser (vqvae_zc.py, Quantize.forward_ with continuous_relax=True: soft :55-60, hard :61-65,
+ * the KL :89-90, gumbel_softmax :284-346).  Row r of the fp32 scores s [rows, ld] is z_r . E (the split3 GEMM of the
+ * nearest-code path) and e2 [K] is |e_j|^2, so a_rj = 2 s_rj - e2_j is -dist up to the row constant |z_r|^2, which
+ * cancels in every softmax and arg-max.  K % 4 == 0; row indices row0 + r < 2^32.  One CTA per row, every reduction
+ * in a fixed order: equal inputs give equal bits.
+ *   cv_gumbel_noise: the noise g[r, j] = -log(-log(u)) of absolute row row0 + r and code j, u in [2^-24, 1 - 2^-24]
+ *     from Philox4x32-10 under `seed`; a function of (seed, absolute row, code) alone.  out: [rows, K] fp32.
+ *   cv_vq_gumbel_fwd: y = softmax((a + g) / tau) (:333-334), written as bf16 (y_f32 = 0) or fp32 (y_f32 = 1) rows of
+ *     stride ldy, or not at all (y = NULL: the hard relaxation needs only the index); idx = the arg-max of (a + g) / tau,
+ *     the lowest index on ties (:338, :345); kl[r] = sum_j qy_j log(qy_j K + 1e-20) with qy = softmax(a) (:89-90),
+ *     or NULL.
+ *   cv_vq_gumbel_bwd: from dy = dL/dy [rows, lddy] fp32 (NULL: no y term) and kl_scale = dL/d(KL mean) / total rows
+ *     (0: no KL term), da = y (dy - <y, dy>) / tau + kl_scale qy (h - <qy, h>) with
+ *     h_j = log(qy_j K + 1e-20) + qy_j K / (qy_j K + 1e-20), written as bf16 [rows, ldda]; rowsum[r] = sum_j da_rj
+ *     (fp32, before rounding), for the -2 z rowsum(da) term of d(-dist)/dz.  y and qy are regenerated from s and the
+ *     noise, so nothing but z needs to be kept between the forward and the backward.
+ * ---------------------------------------------------------------------------------------------- */
+int cv_gumbel_noise(uint64_t seed, int64_t row0, int64_t rows, int K, float* out, void* stream);
+int cv_vq_gumbel_fwd(const float* s, int64_t ld, const float* e2, int64_t rows, int K, uint64_t seed, int64_t row0,
+                     float tau, void* y, int y_f32, int64_t ldy, int64_t* idx, float* kl, void* stream);
+int cv_vq_gumbel_bwd(const float* s, int64_t ld, const float* e2, int64_t rows, int K, uint64_t seed, int64_t row0,
+                     float tau, const float* dy, int64_t lddy, float kl_scale, void* da, int64_t ldda, float* rowsum,
+                     void* stream);
+
 #ifdef __cplusplus
 }
 #endif
