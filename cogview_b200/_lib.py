@@ -95,6 +95,7 @@ def _declare(lib):
         "cv_attn_sparse_bwd_dropout": [P, L, L, P, L, L, P, L, L, P, P, P, P, P, P, I, I, I, I, I, I, I, F, P, P],
         "cv_decode_step": [ctypes.POINTER(DecodeStepArgs), P],
         "cv_sample_topk": [P, L, I, I, F, I, ctypes.POINTER(c_int), I, U64, P, P, P, P, L, P, P, P, P, P, P],
+        "cv_vocab_logprob": [P, L, P, L, P, P, P, I, I, I, I, P],
     })
     lib.cv_attn_sparse_workspace_bytes.argtypes = [I, I, I, I]
     lib.cv_attn_sparse_workspace_bytes.restype = L
@@ -123,6 +124,8 @@ def _declare(lib):
     lib.cv_conv_k4s2_wgrad_workspace_bytes.restype = L
     lib.cv_conv1x1_out3_bwd_workspace_bytes.argtypes = [I]
     lib.cv_conv1x1_out3_bwd_workspace_bytes.restype = L
+    lib.cv_vocab_logprob_workspace_bytes.argtypes = [I, I, I]
+    lib.cv_vocab_logprob_workspace_bytes.restype = L
     for name, args in sigs.items():
         fn = getattr(lib, name)
         fn.argtypes = args

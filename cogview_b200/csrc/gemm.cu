@@ -12,28 +12,18 @@
 //   warpgroups 1-2  wgmma consumers: each owns 64 rows of the 128-row tile (m64 x BN x k16, fp32 accumulators in
 //                   registers), then applies bias / activation / dropout / abs-max and stores its rows straight to
 //                   global memory while the producer already streams the next tile's operands into the ring
+// The ring and the main loop live in gemm_ring.cuh, shared with csrc/vocab_logprob.cu.
 #include <cstdlib>
 
 #include "common.cuh"
+#include "gemm_ring.cuh"
 #include "host.h"
 #include "../../include/cogview_b200.h"
 
 namespace {
 
 using namespace cv;
-
-constexpr int BM = 128;
-constexpr int BK = 64;
-constexpr int NUM_THREADS = 384;
-
-template <int BN>
-struct Cfg {
-    static constexpr int A_BYTES = BM * BK * 2;
-    static constexpr int B_BYTES = BN * BK * 2;
-    static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int STAGES = (BN == 256) ? 4 : 6;
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-};
+using namespace cv::ring;
 
 struct GemmParams {
     int M, N, K;
@@ -81,13 +71,6 @@ __device__ __forceinline__ void dropout2(const DropoutArgs& d, uint64_t idx, flo
     b = rb >= d.threshold ? b * d.scale : 0.f;
 }
 
-template <int N, int TA, int TB>
-__device__ __forceinline__ void mma_n(float* acc, uint64_t da, uint64_t db, uint32_t sc) {
-    if constexpr (N == 256) wgmma_ss_n256<TA, TB>(*reinterpret_cast<float(*)[128]>(acc), da, db, sc);
-    else if constexpr (N == 128) wgmma_ss_n128<TA, TB>(*reinterpret_cast<float(*)[64]>(acc), da, db, sc);
-    else wgmma_ss_n64<TA, TB>(*reinterpret_cast<float(*)[32]>(acc), da, db, sc);
-}
-
 __device__ __forceinline__ void store_pair(__nv_bfloat16* dst, float a, float b, bool pair) {
     if (pair) *reinterpret_cast<uint32_t*>(dst) = pack_bf16x2(a, b);
     else dst[0] = __float2bfloat16_rn(a);
@@ -100,62 +83,24 @@ __device__ __forceinline__ void store_pair(float* dst, float a, float b, bool pa
 template <int BN, bool A_MN, bool B_MN, bool OUT_F32>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
-    using C = Cfg<BN>;
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::STAGES * C::STAGE_BYTES);
-    uint64_t* full_bar = bars;                       // [STAGES]
-    uint64_t* empty_bar = bars + C::STAGES;          // [STAGES]: one arrive per consumer warp
+    const Ring<BN> ring(smem_raw);
 
     const int wg = threadIdx.x >> 7;
     const int tid = threadIdx.x & 127;
     const int num_tiles = p.num_tiles;
 
-    if (threadIdx.x == 0) {
-        tma_prefetch_desc(&tmA);
-        tma_prefetch_desc(&tmB);
-        for (int i = 0; i < C::STAGES; ++i) {
-            mbar_init(&full_bar[i], 1);
-            mbar_init(&empty_bar[i], 8);
-        }
-        fence_barrier_init();
-    }
+    if (threadIdx.x == 0) ring.init(&tmA, &tmB);
     __syncthreads();
 
     if (wg == 0) {
         // ------------------------------ TMA producer ------------------------------
         setmaxnreg_dec<40>();
         if (tid == 0) {
-            int stage = 0;
-            uint32_t phase = 0;
+            RingPos pos;
             for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
                 const TileCoord tc = tile_coord<BN>(p, tile);
-                const int m0 = tc.m0, n0 = tc.n0;
-                for (int kb = 0; kb < p.num_k_blocks; ++kb) {
-                    mbar_wait<false>(&empty_bar[stage], phase ^ 1);
-                    uint8_t* sA = smem + stage * C::STAGE_BYTES;
-                    uint8_t* sB = sA + C::A_BYTES;
-                    mbar_expect_tx(&full_bar[stage], C::A_BYTES + tc.width * BK * 2);
-                    if (!A_MN) {
-                        tma_load_2d(sA, &tmA, &full_bar[stage], kb * BK, m0);
-                    } else {
-#pragma unroll
-                        for (int i = 0; i < BM / 64; ++i)
-                            tma_load_2d(sA + i * (BK * 128), &tmA, &full_bar[stage], m0 + i * 64, kb * BK);
-                    }
-                    if (!B_MN) {    // boxes of 128 rows: one per half tile
-#pragma unroll
-                        for (int i = 0; i < BN / 128; ++i)
-                            if (i * 128 < tc.width)
-                                tma_load_2d(sB + i * (128 * BK * 2), &tmB, &full_bar[stage], kb * BK, n0 + i * 128);
-                    } else {
-#pragma unroll
-                        for (int i = 0; i < BN / 64; ++i)
-                            if (i * 64 < tc.width)
-                                tma_load_2d(sB + i * (BK * 128), &tmB, &full_bar[stage], n0 + i * 64, kb * BK);
-                    }
-                    if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-                }
+                load_tile<BN, A_MN, B_MN>(ring, pos, &tmA, &tmB, tc.m0, tc.n0, tc.width, p.num_k_blocks);
             }
         }
     } else {
@@ -165,44 +110,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         const int warp = tid >> 5, lane = tid & 31;
         const int r_in = 64 * half + 16 * warp + (lane >> 2);   // this thread's rows: r_in and r_in + 8
         const int c_in = 2 * (lane & 3);                    // and columns 8i + c_in, + 1
-        // K-major: 8-row groups 1024 B apart. MN-major: 64-element chunks one TMA box (BK*128 B) apart,
-        // 8-row K groups 1024 B apart.
-        constexpr uint32_t A_LBO = A_MN ? BK * 128 : 0, B_LBO = B_MN ? BK * 128 : 0;
-        constexpr uint32_t A_KSTEP = A_MN ? 16 * 128 : 32, B_KSTEP = B_MN ? 16 * 128 : 32;
-        const uint32_t a_half = A_MN ? half * (BK * 128) : half * (64 * 128);
-        constexpr int TA = A_MN ? 1 : 0, TB = B_MN ? 1 : 0;
-        int stage = 0;
-        uint32_t phase = 0;
+        RingPos pos;
         float acc[BN / 2];
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
         for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
             const TileCoord tc = tile_coord<BN>(p, tile);
-            const bool full = tc.width == BN;
-            int prev = -1;
-            for (int kb = 0; kb < p.num_k_blocks; ++kb) {
-                mbar_wait<false>(&full_bar[stage], phase);
-                const uint32_t a_addr = smem_u32(smem + stage * C::STAGE_BYTES) + a_half;
-                const uint32_t b_addr = smem_u32(smem + stage * C::STAGE_BYTES + C::A_BYTES);
-                fence_regs(acc);
-                wgmma_fence();
-#pragma unroll
-                for (int k = 0; k < BK / 16; ++k) {
-                    const uint64_t da = make_smem_desc_sw128(a_addr + k * A_KSTEP, A_LBO, 1024);
-                    const uint64_t db = make_smem_desc_sw128(b_addr + k * B_KSTEP, B_LBO, 1024);
-                    const uint32_t sc = (kb | k) != 0 ? 1u : 0u;
-                    if (full) mma_n<BN, TA, TB>(acc, da, db, sc);
-                    else mma_n<BN / 2, TA, TB>(acc, da, db, sc);
-                }
-                wgmma_commit();
-                wgmma_wait<1>();                            // the previous k-block's MMAs retired: free its slot
-                if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
-                prev = stage;
-                if (++stage == C::STAGES) { stage = 0; phase ^= 1; }
-            }
-            wgmma_wait<0>();
-            fence_regs(acc);
-            if (lane == 0) mbar_arrive(&empty_bar[prev]);
+            mma_tile<BN, A_MN, B_MN>(ring, pos, acc, half, lane, tc.width == BN, p.num_k_blocks);
 
             const int m0 = tc.m0, n0 = tc.n0;
             float tmax = 0.f;

@@ -2,12 +2,15 @@
 UnifiedTokenizer.parse_query / DecodeIds (data_utils/unified_tokenizer.py:91-196): query templates per task, query
 assembly from already-tokenised text and image codes, beam batching, and decoding of the generated image codes
 through the VQ-VAE.  Text <-> string conversion (sentencepiece) and image file I/O stay with the caller."""
+from collections import namedtuple
+
 import torch
 
 from . import vqvae
 from .generation.magnify import magnify, magnify_batch
 from .generation.sampling import (add_interlacing_beam_marks, filling_sequence, filling_sequences,
-                                  filling_shared_prompts, get_tokenizer, inverse_prompt_score)
+                                  filling_shared_prompts, get_tokenizer, inverse_prompt_score,
+                                  inverse_prompt_scores)
 
 # generate_samples.py:203-214
 QUERY_TEMPLATES = {
@@ -251,3 +254,35 @@ def post_selection(model, args, seq, score=inverse_prompt_score):
     model.eval()
     with torch.no_grad():
         return torch.cat([score(model, seq[i * mbz:(i + 1) * mbz], args) for i in range(max(num // mbz, 1))], dim=0)
+
+
+Reranked = namedtuple('Reranked', ['index', 'rows', 'images', 'scores', 'all_scores'])
+Reranked.__doc__ = """The `keep` best of one caption's candidates, best first: index [keep] into its `num` draws, their
+token rows [keep, len], images [keep, 3, H, W] and scores [keep], and the scores of all draws, all_scores [num].
+index, scores and all_scores are on the CPU; rows and images stay where generation left them."""
+
+
+def rerank(model, caption_model, vq_model, args, seqs, num, keep):
+    """CogView's draw-many-keep-the-best recipe (generate_samples.py:147-200, 246-270) end to end, for many captions.
+    seqs: 'text2image' templates, one per caption ([ROI1] caption [BASE] [BOI1] [MASK]*1024, 1-D LongTensors).
+    `num` images per caption come from generate_images_batch with `model`; each is scored by `caption_model` (which may
+    be `model` itself) as the log-likelihood of its caption given the image — the post-selection queries of all
+    captions go through inverse_prompt_scores together, in groups of args.max_inference_batch_size rows.  Returns one
+    Reranked per caption, holding its `keep` best candidates ordered by descending score, ties to the lower index."""
+    assert 1 <= keep <= num
+    tok = get_tokenizer(args)
+    n_img = tok.img_tokenizer.num_tokens
+    drawn = generate_images_batch(model, vq_model, args, seqs, num=num)
+    queries = []
+    for seq, (rows, _) in zip(seqs, drawn):
+        text = [x + n_img for x in caption_ids(seq, tok)]
+        queries.extend(post_selection_rows(rows, text, tok).unbind(0))
+    caption_model.eval()
+    scores = inverse_prompt_scores(caption_model, queries, args).cpu()
+    out = []
+    for c, (rows, imgs) in enumerate(drawn):
+        s = scores[c * num:(c + 1) * num]
+        index = torch.sort(s, descending=True, stable=True).indices[:keep]
+        dev = index.to(rows.device)
+        out.append(Reranked(index, rows[dev], imgs[index.to(imgs.device)], s[index], s))
+    return out

@@ -549,3 +549,48 @@ def inverse_prompt_score(model, seq, args):
     pred = log_probs[:, botext:-1, :]
     target = tokens[:, botext + 1:].unsqueeze(-1)
     return torch.gather(pred, dim=2, index=target).squeeze(-1).sum(dim=-1)
+
+
+def inverse_prompt_scores(model, seqs, args):
+    """inverse_prompt_score for many post-selection rows at once, on GPT2Model.token_logprobs: the caption
+    log-likelihood given the image of every row, fp32 [N] in input order.  seqs: a 2-D LongTensor or a list of 1-D
+    rows ([BASE] [BOI1] 1024 codes [EOI1] [ROI1] caption); rows may belong to different captions, so their lengths may
+    differ.  Rows go through the model in groups of at most args.max_inference_batch_size, each group padded at the
+    end with [PAD] (causal attention keeps the padding out of every scored position).  Each caption token is scored
+    over the vocabulary window [img_tokenizer.num_tokens, V), the window the reference's -inf mask leaves.  No logits
+    and no K|V cache are kept.  The abs-max LayerNorm scale is one scalar per forward tensor, so a row of a mixed or
+    padded group matches a run of that row alone within bf16 tolerance, not bit for bit; where the reference's fp32
+    log(softmax) underflows to -inf, this returns the finite log-probability.  Dense attention (is_sparse=0) only."""
+    if getattr(args, 'is_sparse', 0) != 0:
+        raise NotImplementedError('inverse_prompt_scores supports dense attention (is_sparse=0) only')
+    tokenizer = get_tokenizer(args)
+    rows = list(seqs.unbind(0)) if torch.is_tensor(seqs) else list(seqs)
+    botext = 2 + 1024 + 1
+    assert all(r.dim() == 1 and r.shape[0] > botext + 1 for r in rows), 'post-selection rows hold a caption'
+    n = len(rows)
+    mbz = max(1, args.max_inference_batch_size)
+    n_img = tokenizer.img_tokenizer.num_tokens
+    pad, roi1 = tokenizer['[PAD]'], tokenizer['[ROI1]']
+    out = []
+    with torch.no_grad():
+        for g0 in range(0, n, mbz):
+            group = rows[g0:g0 + mbz]
+            device = group[0].device
+            lens = [r.shape[0] for r in group]
+            L = max(lens)
+            tokens = torch.full((len(group), L), pad, dtype=torch.long, device=device)
+            for i, r in enumerate(group):
+                tokens[i, :lens[i]] = r.to(device)
+            assert bool((tokens[:, botext] == roi1).all()), 'post-selection rows have [ROI1] at index %d' % botext
+            attention_mask, _, position_ids = get_masks_and_position_ids(tokens)
+            # row i scores positions botext .. lens[i] - 2, each predicting the token after it
+            ncap = torch.tensor([n_ - 1 - botext for n_ in lens], device=device)
+            col = torch.arange(max(lens) - 1 - botext, device=device).view(1, -1)
+            valid = col < ncap.view(-1, 1)
+            flat = (torch.arange(len(group), device=device).view(-1, 1) * L + botext + col)[valid]
+            lp = model.token_logprobs(tokens, position_ids, attention_mask, flat, tokens.view(-1)[flat + 1],
+                                      vocab_begin=n_img)
+            per_pos = torch.zeros(valid.shape, dtype=torch.float32, device=lp.device)
+            per_pos[valid.to(lp.device)] = lp
+            out.append(per_pos.sum(dim=1))        # in position order per row: no atomics, the same sum every call
+    return torch.cat(out, dim=0)

@@ -261,6 +261,36 @@ def _chunk_run_impl(self, tokens, position_ids, mems, row_pad=None):
 GPT2Model.chunk_run = _chunk_run_impl
 
 
+def _token_logprobs_impl(self, input_ids, position_ids, attention_mask, score_index, targets, vocab_begin=0,
+                         vocab_end=None, *, is_sparse=0):
+    """log_softmax over the vocabulary window [vocab_begin, vocab_end) of the logits at a few positions, picked at
+    their targets: what generation/sampling.py:214-230 reads of a full forward, without the forward's logits or
+    memory.  input_ids, position_ids int64 [b, s]; attention_mask as forward takes it; score_index int64 flat
+    indices into the b*s rows; targets int64 [len(score_index)] (a target outside the window gives -inf).  Returns
+    fp32 [len(score_index)].  The layers run with no memory kept (run_layers(keep_mems=False): no K|V cache is
+    prepared and the pooled caches stay as they are); only the scored rows of the bf16 final-LN output go through
+    cv_vocab_logprob, which never writes a logit to memory.  torch.no_grad() and dense attention (is_sparse=0) only."""
+    if torch.is_grad_enabled():
+        raise RuntimeError('token_logprobs runs under torch.no_grad() only')
+    if is_sparse != 0:
+        raise NotImplementedError('token_logprobs supports dense attention (is_sparse=0) only')
+    tr = self.transformer
+    b, sq = input_ids.shape
+    sep = mask_to_sep(attention_mask, sq, sq)
+    if position_ids.shape != input_ids.shape:
+        position_ids = position_ids.expand_as(input_ids)
+    wte, wpe = self.word_embeddings.weight, tr.position_embeddings.weight
+    w = _as_bf16(wte.detach()).contiguous()
+    am_x = ops.new_scalars(1, wte.device)
+    x = ops.embed_fwd(input_ids, position_ids, w, _as_bf16(wpe.detach()).contiguous(), am_x)
+    y, _ = tr.run_layers(x, am_x, b, sq, sep, [], keep_mems=False)
+    rows = y.index_select(0, score_index.to(device=y.device, dtype=torch.long).view(-1))
+    return ops.vocab_logprob(rows, w, targets.to(device=y.device, dtype=torch.long), vocab_begin, vocab_end)
+
+
+GPT2Model.token_logprobs = _token_logprobs_impl
+
+
 class _NoCtx:
     def save_for_backward(self, *a):
         pass

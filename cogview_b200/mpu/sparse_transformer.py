@@ -601,13 +601,15 @@ class GPT2ParallelTransformer(torch.nn.Module):
                          dim=-1)
 
     def run_layers(self, x, am_x, b, sq, sep, mems, word_embedding_weight=None, is_sparse=0, txt_indices_bool=None,
-                   img_indices_bool=None, chunk_attn=None):
+                   img_indices_bool=None, chunk_attn=None, keep_mems=True):
         """x fp32 [b*sq, h].  Returns (final-LN output bf16 [b*sq, h], mem_layers list).
         chunk_attn (K|V-cache mode only): None, or a callable (layer index, caches) -> attention hook that reads the
-        layer's cache and appends the new tokens' K|V itself (rows at their own cache lengths, GPT2Model.chunk_run)."""
+        layer's cache and appends the new tokens' K|V itself (rows at their own cache lengths, GPT2Model.chunk_run).
+        keep_mems=False: no memory at all, whatever max_memory_length says — no K|V cache is prepared or touched and
+        mem_layers is empty (a forward whose states are never decoded from, GPT2Model.token_logprobs)."""
         from . import kv_cache
         h = self.hidden_size
-        keep_mems = self.max_memory_length > 0
+        keep_mems = keep_mems and self.max_memory_length > 0
         mode = self.mems_mode if keep_mems else None
         if mems and torch.is_grad_enabled() and x.requires_grad:
             raise NotImplementedError('training with memory is not supported')

@@ -281,6 +281,29 @@ def cross_entropy_bwd(logits, target, rmax, rsum, grad_loss):
     return dl[:, :V]
 
 
+def vocab_logprob(h, w, target, v_begin=0, v_end=None):
+    """log_softmax(h @ w[v_begin:v_end]^T)[m, target[m] - v_begin] for every row m, without materialising the logits:
+    h bf16 [M, K], w bf16 [V, K] (the tied word embedding), target int64 [M] (absolute vocabulary ids; one outside
+    [v_begin, v_end) gives -inf).  Returns fp32 [M]."""
+    require_cuda(h, w, target)
+    assert h.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and h.dim() == 2 and w.dim() == 2
+    assert h.stride(1) == 1 and w.stride(1) == 1 and h.shape[1] == w.shape[1]
+    M, K = h.shape
+    v_end = w.shape[0] if v_end is None else v_end
+    assert 0 <= v_begin < v_end <= w.shape[0], "vocabulary window [%d, %d) outside [0, %d)" % (v_begin, v_end,
+                                                                                            w.shape[0])
+    target = target.contiguous().view(-1)
+    assert target.dtype == torch.int64 and target.numel() == M
+    out = torch.empty(M, dtype=torch.float32, device=h.device)
+    if M == 0:
+        return out
+    ws = torch.empty(lib().cv_vocab_logprob_workspace_bytes(M, v_begin, v_end) // 4, dtype=torch.float32,
+                     device=h.device)
+    check(lib().cv_vocab_logprob(ptr(h), h.stride(0), ptr(w), w.stride(0), ptr(target), ptr(out), ptr(ws), M, K,
+                                 int(v_begin), int(v_end), stream_ptr()), "cv_vocab_logprob")
+    return out
+
+
 def gelu_bwd(pre, dact):
     require_cuda(pre, dact)
     assert pre.is_contiguous() and dact.is_contiguous() and pre.dtype == torch.bfloat16 and dact.dtype == torch.bfloat16

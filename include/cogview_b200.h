@@ -463,6 +463,20 @@ int cv_vq_gumbel_bwd(const float* s, int64_t ld, const float* e2, int64_t rows, 
                      float tau, const float* dy, int64_t lddy, float kl_scale, void* da, int64_t ldda, float* rowsum,
                      void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Token log-probabilities over a vocabulary window, without logits in global memory (post-selection: the caption
+ * log-likelihood of generation/sampling.py:214-230, log(softmax) of the logits with the image vocabulary at -inf).
+ *   logp[m] = H[m] . W[target[m]] - logsumexp_{v_begin <= v < v_end} H[m] . W[v]; -inf when target[m] lies outside
+ *   [v_begin, v_end).  H bf16 [M, K] (ldh), W bf16 [V >= v_end, K] (ldw; the tied word embedding), target int64 [M],
+ *   logp fp32 [M].  K, ldh and ldw follow cv_gemm_bf16 (multiples of 8); M >= 1 and the window width are arbitrary.
+ *   A wgmma GEMM whose epilogue keeps one (max, sum exp) pair per (row, 256-column tile), then one reduction per row
+ *   in column-tile order: equal inputs give equal bits.  workspace: cv_vocab_logprob_workspace_bytes(M, v_begin,
+ *   v_end) bytes, 8-byte aligned, need not be initialised.
+ * ---------------------------------------------------------------------------------------------- */
+int64_t cv_vocab_logprob_workspace_bytes(int M, int v_begin, int v_end);
+int cv_vocab_logprob(const void* H, int64_t ldh, const void* W, int64_t ldw, const int64_t* target, float* logp,
+                     float* workspace, int M, int K, int v_begin, int v_end, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
