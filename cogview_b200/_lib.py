@@ -96,6 +96,9 @@ def _declare(lib):
         "cv_decode_step": [ctypes.POINTER(DecodeStepArgs), P],
         "cv_sample_topk": [P, L, I, I, F, I, ctypes.POINTER(c_int), I, U64, P, P, P, P, L, P, P, P, P, P, P],
         "cv_vocab_logprob": [P, L, P, L, P, P, P, I, I, I, I, P],
+        "cv_vocab_xent_fwd": [P, L, P, L, P, P, P, P, I, I, I, P],
+        "cv_vocab_xent_dlogits": [P, L, P, L, P, P, P, P, L, I, I, I, I, P],
+        "cv_add_f32": [P, P, L, P],
     })
     lib.cv_attn_sparse_workspace_bytes.argtypes = [I, I, I, I]
     lib.cv_attn_sparse_workspace_bytes.restype = L
@@ -126,6 +129,8 @@ def _declare(lib):
     lib.cv_conv1x1_out3_bwd_workspace_bytes.restype = L
     lib.cv_vocab_logprob_workspace_bytes.argtypes = [I, I, I]
     lib.cv_vocab_logprob_workspace_bytes.restype = L
+    lib.cv_vocab_xent_workspace_bytes.argtypes = [I, I]
+    lib.cv_vocab_xent_workspace_bytes.restype = L
     for name, args in sigs.items():
         fn = getattr(lib, name)
         fn.argtypes = args

@@ -236,6 +236,18 @@ __global__ void gelu_bwd_kernel(const __nv_bfloat16* __restrict__ pre, const __n
 }
 
 // ------------------------------------------------------------------------------------------------
+// dst += src (fp32): the chunk sum of the fused cross-entropy's dH (model/gpt2_modeling.py _VocabXentFn)
+// ------------------------------------------------------------------------------------------------
+__global__ void add_f32_kernel(float* __restrict__ dst, const float* __restrict__ src, size_t n4) {
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
+        float4 a = reinterpret_cast<float4*>(dst)[i];
+        const float4 b = reinterpret_cast<const float4*>(src)[i];
+        a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
+        reinterpret_cast<float4*>(dst)[i] = a;
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // Column sums: db[c] = sum_r dy[r, c]   (bias gradients of the four linears)
 // ------------------------------------------------------------------------------------------------
 constexpr int COLSUM_SPLITS = 32;
@@ -340,6 +352,17 @@ extern "C" int cv_cross_entropy_bwd(const float* logits, int64_t ld, const int64
     CV_REQUIRE(rows > 0 && vocab > 0 && ld % 4 == 0 && ldd % 4 == 0, "ld/ldd must be multiples of 4");
     ce_bwd_kernel<<<rows, CE_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
         logits, ld, target, row_max, row_sum, grad_loss, static_cast<__nv_bfloat16*>(dlogits), ldd, vocab);
+    CV_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" int cv_add_f32(float* dst, const float* src, int64_t n, void* stream) {
+    CV_REQUIRE(dst && src, "null pointer");
+    CV_REQUIRE(n > 0 && n % 4 == 0, "element count must be a positive multiple of 4");
+    CV_REQUIRE(((reinterpret_cast<uintptr_t>(dst) | reinterpret_cast<uintptr_t>(src)) & 15) == 0,
+               "dst and src must be 16-byte aligned");
+    add_f32_kernel<<<grid_for((size_t)n / 4, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(dst, src,
+                                                                                               (size_t)n / 4);
     CV_LAUNCH_CHECK();
     return 0;
 }

@@ -59,6 +59,30 @@ class _LogitsFn(torch.autograd.Function):
         return d_hidden, d_w.to(ctx.wdtype)
 
 
+class _VocabXentFn(torch.autograd.Function):
+    """Per-token loss = logsumexp(h W^T) - (h W^T)[target] with the tied word-embedding matrix, without the fp32
+    logits: the values vocab_parallel_cross_entropy(_LogitsFn(h, W), target) gives, from the same fp32 GEMM
+    accumulators (only the order of the sum of exponentials differs).  The forward keeps h, the bf16 weight, the
+    targets and the row log-sum-exp; the backward recomputes the logits one vocabulary chunk at a time
+    (ops.vocab_xent_bwd: bf16 dlogits as in the logits route, dH summed over chunks in fp32 when there are several,
+    dW written per chunk) and never holds an [M, V] tensor.  Repeats with equal inputs and budget are bit-equal."""
+
+    @staticmethod
+    def forward(ctx, hidden, weight, target, chunk_bytes):
+        w = _as_bf16(weight)
+        loss, lse = ops.vocab_xent_fwd(hidden, w, target)
+        ctx.save_for_backward(hidden, w, target, lse)
+        ctx.wdtype = weight.dtype
+        ctx.chunk_bytes = chunk_bytes
+        return loss
+
+    @staticmethod
+    def backward(ctx, grad_loss):
+        hidden, w, target, lse = ctx.saved_tensors
+        d_hidden, d_w = ops.vocab_xent_bwd(hidden, w, target, lse, grad_loss, ctx.chunk_bytes)
+        return d_hidden, d_w.to(ctx.wdtype), None, None
+
+
 class GPT2Model(torch.nn.Module):
     """GPT-2 language model over concatenated text + image tokens.  forward returns (logits, *mems)."""
 
@@ -76,17 +100,25 @@ class GPT2Model(torch.nn.Module):
             checkpoint_num_layers, query_window=query_window, key_window_times=key_window_times, num_pivot=num_pivot)
 
     def forward(self, input_ids, position_ids, attention_mask, txt_indices_bool, img_indices_bool, is_sparse, *mems,
-                logits_last_only=False):
+                logits_last_only=False, labels=None, xent_chunk_bytes=None):
         """Same positional arguments as the reference (model/gpt2_modeling.py:106).  Returns
         (logits [b, s, V] fp32, *mems).  `logits_last_only` (keyword, extension): only the last position's
-        logits are computed — what the sampling loop reads (generation/sampling.py:155)."""
+        logits are computed — what the sampling loop reads (generation/sampling.py:155).
+        `labels` (keyword, extension; int64 [b, s]): returns (losses [b, s] fp32, *mems) instead, the per-token
+        loss vocab_parallel_cross_entropy(logits.float(), labels) gives, computed without the logits
+        (_VocabXentFn; with and without autograd, never on the decode fast path).  The backward's dlogits chunk
+        budget is `xent_chunk_bytes` (default ops.XENT_CHUNK_BYTES).  A label outside [0, V) gives a NaN loss."""
+        if labels is not None and logits_last_only:
+            raise ValueError('labels= and logits_last_only=True cannot be combined: the loss needs every position')
         tr = self.transformer
         b, sq = input_ids.shape
+        if labels is not None and tuple(labels.shape) != (b, sq):
+            raise ValueError('labels must have the shape of input_ids %s, got %s' % ((b, sq), tuple(labels.shape)))
         mem_len = mems[0].size(1) if mems else 0
         sep = 0 if is_sparse != 0 else mask_to_sep(attention_mask, sq, sq + mem_len)
         if position_ids.shape != input_ids.shape:
             position_ids = position_ids.expand_as(input_ids)
-        fast = self._fast_decode(input_ids, position_ids, mems, b, sq) if is_sparse == 0 else None
+        fast = self._fast_decode(input_ids, position_ids, mems, b, sq) if is_sparse == 0 and labels is None else None
         if fast is not None:
             return fast
         wte, wpe = self.word_embeddings.weight, tr.position_embeddings.weight
@@ -99,6 +131,13 @@ class GPT2Model(torch.nn.Module):
                               _as_bf16(wpe.detach()).contiguous(), am_x)
         y, mem_layers = tr.run_layers(x, am_x, b, sq, sep, mems, is_sparse=is_sparse,
                                       txt_indices_bool=txt_indices_bool, img_indices_bool=img_indices_bool)
+        if labels is not None:
+            target = labels.reshape(-1).to(device=y.device, dtype=torch.long)
+            if torch.is_grad_enabled() and (y.requires_grad or wte.requires_grad):
+                losses = _VocabXentFn.apply(y, wte, target, xent_chunk_bytes)
+            else:
+                losses, _ = ops.vocab_xent_fwd(y, _as_bf16(wte.detach()), target)
+            return (losses.view(b, sq), *mem_layers)
         h = y.shape[1]
         if logits_last_only:
             y = y.view(b, sq, h)[:, -1].contiguous()

@@ -304,6 +304,111 @@ def vocab_logprob(h, w, target, v_begin=0, v_end=None):
     return out
 
 
+# Byte budget of one bf16 dlogits chunk [M, width] in the fused cross-entropy backward (vocab_xent_bwd): the largest
+# tensor it allocates.  256 MiB holds the whole 58240-column vocabulary for up to 2304 rows (2 x 1088 tokens fit).
+XENT_CHUNK_BYTES = 256 << 20
+
+
+def xent_chunks(M, V, chunk_bytes=None):
+    """Column windows [(v0, v1), ...] of the fused backward, in order and covering [0, V): one window when the bf16
+    dlogits of all V columns (rows padded to 8 columns) fit `chunk_bytes` (default XENT_CHUNK_BYTES), else windows
+    of the largest multiple of 256 columns that fits (at least 256), the last one taking the remainder."""
+    budget = XENT_CHUNK_BYTES if chunk_bytes is None else int(chunk_bytes)
+    if M * ((V + 7) // 8 * 8) * 2 <= budget:
+        return [(0, V)]
+    width = max(256, budget // (2 * M) // 256 * 256)
+    return [(v0, min(V, v0 + width)) for v0 in range(0, V, width)]
+
+
+def add_f32(dst, src):
+    """dst += src (fp32, contiguous, same number of elements, a multiple of 4)."""
+    require_cuda(dst, src)
+    assert dst.dtype == torch.float32 and src.dtype == torch.float32 and dst.is_contiguous() and src.is_contiguous()
+    assert dst.numel() == src.numel()
+    check(lib().cv_add_f32(ptr(dst), ptr(src), dst.numel(), stream_ptr()), "cv_add_f32")
+    return dst
+
+
+def _xent_args(h, w, target):
+    require_cuda(h, w, target)
+    assert h.dtype == torch.bfloat16 and w.dtype == torch.bfloat16 and h.dim() == 2 and w.dim() == 2
+    assert h.stride(1) == 1 and w.stride(1) == 1 and h.shape[1] == w.shape[1]
+    target = target.contiguous().view(-1)
+    assert target.dtype == torch.int64 and target.numel() == h.shape[0]
+    return target
+
+
+def vocab_xent_fwd(h, w, target):
+    """Per-token cross-entropy over the whole vocabulary without logits in memory: h bf16 [M, K] (the final
+    LayerNorm's output), w bf16 [V, K] (the tied word embedding), target int64 [M].  Returns (loss, lse), fp32 [M]:
+    loss = lse - h . w[target], lse = logsumexp(h @ w^T) per row, from the same fp32 GEMM accumulators the logits
+    route rounds; only the order of the sum of exponentials differs.  A target outside [0, V) gives loss NaN.  Equal
+    inputs give equal bits."""
+    target = _xent_args(h, w, target)
+    M, K = h.shape
+    V = w.shape[0]
+    loss = torch.empty(M, dtype=torch.float32, device=h.device)
+    lse = torch.empty(M, dtype=torch.float32, device=h.device)
+    if M == 0:
+        return loss, lse
+    ws = torch.empty(lib().cv_vocab_xent_workspace_bytes(M, V) // 4, dtype=torch.float32, device=h.device)
+    check(lib().cv_vocab_xent_fwd(ptr(h), h.stride(0), ptr(w), w.stride(0), ptr(target), ptr(loss), ptr(lse), ptr(ws),
+                                  M, K, V, stream_ptr()), "cv_vocab_xent_fwd")
+    return loss, lse
+
+
+def vocab_xent_dlogits(h, w, target, lse, grad_loss, v_begin, v_end, out=None):
+    """bf16 [M, v_end - v_begin] = grad_loss[m] * (softmax(h @ w^T)[m, v] - [v == target[m]]) for v in
+    [v_begin, v_end), recomputing the logits of the window; lse from vocab_xent_fwd.  `out` (bf16 [M, >= width],
+    last dim contiguous, even row stride) receives it in its first v_end - v_begin columns."""
+    target = _xent_args(h, w, target)
+    M, K = h.shape
+    assert 0 <= v_begin < v_end <= w.shape[0], "vocabulary window [%d, %d) outside [0, %d)" % (v_begin, v_end,
+                                                                                            w.shape[0])
+    n = v_end - v_begin
+    if out is None:
+        out = torch.empty((M, (n + 7) // 8 * 8), dtype=torch.bfloat16, device=h.device)[:, :n]
+    require_cuda(lse, grad_loss, out)
+    assert out.dtype == torch.bfloat16 and out.stride(1) == 1 and out.shape[0] == M and out.shape[1] >= n
+    assert lse.dtype == torch.float32 and lse.is_contiguous() and lse.numel() == M
+    grad_loss = grad_loss.reshape(-1).float().contiguous()
+    assert grad_loss.numel() == M
+    check(lib().cv_vocab_xent_dlogits(ptr(h), h.stride(0), ptr(w), w.stride(0), ptr(target), ptr(lse), ptr(grad_loss),
+                                      ptr(out), out.stride(0), M, K, int(v_begin), int(v_end), stream_ptr()),
+          "cv_vocab_xent_dlogits")
+    return out[:, :n]
+
+
+def vocab_xent_bwd(h, w, target, lse, grad_loss, chunk_bytes=None):
+    """Backward of vocab_xent_fwd, never holding [M, V]: for each column window [v0, v1) of xent_chunks(M, V,
+    chunk_bytes), D = vocab_xent_dlogits (bf16, as the logits route's dlogits), dW[v0:v1] = D^T h (the wgrad GEMM,
+    written in place) and dH += D w[v0:v1] (the dgrad GEMM).  Returns (dH bf16 [M, K], dW bf16 [V, K]).  With one
+    window dH is the dgrad GEMM's bf16 output, as in the logits route; with several it is summed in fp32 in window
+    order and rounded once.  Equal inputs and budget give equal bits."""
+    target = _xent_args(h, w, target)
+    M, K = h.shape
+    V = w.shape[0]
+    chunks = xent_chunks(M, V, chunk_bytes)
+    widest = max(v1 - v0 for v0, v1 in chunks)
+    d = torch.empty((M, (widest + 7) // 8 * 8), dtype=torch.bfloat16, device=h.device)
+    dw = torch.empty((V, K), dtype=torch.bfloat16, device=h.device)
+    if len(chunks) == 1:
+        dc = vocab_xent_dlogits(h, w, target, lse, grad_loss, 0, V, out=d)
+        dh = gemm(dc, w, b_mn_major=True)
+        gemm(dc, h, a_mn_major=True, b_mn_major=True, out=dw)
+        return dh, dw
+    dh = torch.empty((M, K), dtype=torch.float32, device=h.device)
+    part = torch.empty_like(dh)
+    for i, (v0, v1) in enumerate(chunks):
+        dc = vocab_xent_dlogits(h, w, target, lse, grad_loss, v0, v1, out=d)
+        gemm(dc, h, a_mn_major=True, b_mn_major=True, out=dw[v0:v1])
+        gemm(dc, w[v0:v1], b_mn_major=True, out_dtype=torch.float32, out=dh if i == 0 else part)
+        if i > 0:
+            add_f32(dh, part)
+    del d, dc, part
+    return dh.to(torch.bfloat16), dw
+
+
 def gelu_bwd(pre, dact):
     require_cuda(pre, dact)
     assert pre.is_contiguous() and dact.is_contiguous() and pre.dtype == torch.bfloat16 and dact.dtype == torch.bfloat16

@@ -26,15 +26,22 @@ def weighted_loss(losses, tokens, loss_mask, txt_loss_scale=1.0, img_vocab=None)
     return loss, img_loss, txt_loss
 
 
-def forward_step(batch, model, txt_loss_scale=1.0, is_sparse=0, mems=()):
+def forward_step(batch, model, txt_loss_scale=1.0, is_sparse=0, mems=(), fused_loss=False):
     """pretrain_gpt2.py:292-337 for one `make_batch` tuple.  Returns (loss, mems, img_loss, txt_loss); the logging
-    all-reduce of the partial losses is done when a process group exists."""
+    all-reduce of the partial losses is done when a process group exists.  `fused_loss` computes the per-token
+    losses inside the model (GPT2Model.forward(..., labels=)) without materialising the fp32 logits; the same
+    losses up to the order of the softmax sum, with far less memory in the loss stage."""
     tokens, labels, loss_mask, attention_mask, position_ids = batch
     img_vocab = get_tokenizer().img_tokenizer.num_tokens
     img_indices_bool = tokens.detach() < img_vocab
     txt_indices_bool = (~img_indices_bool) & (loss_mask > 0)
-    logits, *mems = model(tokens, position_ids, attention_mask, txt_indices_bool, img_indices_bool, is_sparse, *mems)
-    losses = mpu.vocab_parallel_cross_entropy(logits.contiguous().float(), labels)
+    if fused_loss:
+        losses, *mems = model(tokens, position_ids, attention_mask, txt_indices_bool, img_indices_bool, is_sparse,
+                              *mems, labels=labels)
+    else:
+        logits, *mems = model(tokens, position_ids, attention_mask, txt_indices_bool, img_indices_bool, is_sparse,
+                              *mems)
+        losses = mpu.vocab_parallel_cross_entropy(logits.contiguous().float(), labels)
     loss, img_loss, txt_loss = weighted_loss(losses, tokens, loss_mask, txt_loss_scale, img_vocab)
     if torch.distributed.is_available() and torch.distributed.is_initialized():
         world = torch.distributed.get_world_size()
@@ -47,10 +54,11 @@ def forward_step(batch, model, txt_loss_scale=1.0, is_sparse=0, mems=()):
 
 
 def train_step(batch, model, optimizer, lr_scheduler=None, txt_loss_scale=1.0, is_sparse=0, mems=(),
-               check_skipped=True):
+               check_skipped=True, fused_loss=False):
     """pretrain_gpt2.py:406-450.  Returns (loss, skipped_iter, mems, img_loss, txt_loss).  `check_skipped` reads the
-    optimizer's device-side skip flag (one small device->host read per step)."""
-    lm_loss, mems, img_loss, txt_loss = forward_step(batch, model, txt_loss_scale, is_sparse, mems)
+    optimizer's device-side skip flag (one small device->host read per step); `fused_loss` as in forward_step."""
+    lm_loss, mems, img_loss, txt_loss = forward_step(batch, model, txt_loss_scale, is_sparse, mems,
+                                                     fused_loss=fused_loss)
     partial = img_loss + txt_loss
     if partial.isnan().any() or partial.isinf().any():
         print('Skipping backward and optimizer step for nan or inf in forwarding!')

@@ -137,6 +137,9 @@ int cv_cross_entropy_bwd(const float* logits, int64_t ld, const int64_t* target,
                          int vocab, void* stream);
 
 /* GELU backward (mpu/sparse_transformer.py:172-176): dpre = dact * gelu'(pre), bf16, n % 8 == 0 */
+/* dst[i] += src[i] for i < n, fp32; n a multiple of 4, both 16-byte aligned. */
+int cv_add_f32(float* dst, const float* src, int64_t n, void* stream);
+
 int cv_gelu_bwd(const void* pre, const void* dact, void* dpre, int64_t n, void* stream);
 /* bias gradient: out[c] = sum_r dy[r, c] (bf16 in/out, fp32 accumulate) */
 int64_t cv_colsum_workspace_bytes(int cols);
@@ -476,6 +479,30 @@ int cv_vq_gumbel_bwd(const float* s, int64_t ld, const float* e2, int64_t rows, 
 int64_t cv_vocab_logprob_workspace_bytes(int M, int v_begin, int v_end);
 int cv_vocab_logprob(const void* H, int64_t ldh, const void* W, int64_t ldw, const int64_t* target, float* logp,
                      float* workspace, int M, int K, int v_begin, int v_end, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Vocabulary cross-entropy for training without logits in global memory: the per-token loss of
+ * mpu/cross_entropy.py:27-104 over the whole vocabulary [0, V), with its gradient recomputed per column window.
+ *   H bf16 [M, K] (ldh), W bf16 [V, K] (ldw; the tied word embedding), target int64 [M]; K, ldh and ldw follow
+ *   cv_gemm_bf16 (multiples of 8, H and W 16-byte aligned); M >= 1 and V are arbitrary.
+ * cv_vocab_xent_fwd: loss[m] = lse[m] - H[m] . W[target[m]], lse[m] = logsumexp_{0 <= v < V} H[m] . W[v], both fp32
+ *   [M], from the fp32 accumulators of a wgmma GEMM (the logits route rounds the same values; only the order of the
+ *   sum of exponentials differs).  A target outside [0, V) gives loss NaN (lse is still written).  workspace:
+ *   cv_vocab_xent_workspace_bytes(M, V) bytes, 8-byte aligned, need not be initialised.  The row's partial
+ *   (max, sum exp) pairs are folded in column-tile order: equal inputs give equal bits.
+ * cv_vocab_xent_dlogits: for the window [v_begin, v_end) (0 <= v_begin < v_end <= V)
+ *   D[m, v - v_begin] = bf16(grad_loss[m] * (exp(H[m] . W[v] - lse[m]) - [v == target[m]])),
+ *   lse from cv_vocab_xent_fwd, grad_loss fp32 [M].  D bf16 [M, ldd], ldd >= v_end - v_begin and even, D 4-byte
+ *   aligned; columns at or past v_end - v_begin and rows past M are not written.  A target outside the window
+ *   subtracts nothing there.  Each element is computed once from a fixed-order GEMM, with no atomics: equal inputs
+ *   give equal bits.
+ * ---------------------------------------------------------------------------------------------- */
+int64_t cv_vocab_xent_workspace_bytes(int M, int V);
+int cv_vocab_xent_fwd(const void* H, int64_t ldh, const void* W, int64_t ldw, const int64_t* target, float* loss,
+                      float* lse, float* workspace, int M, int K, int V, void* stream);
+int cv_vocab_xent_dlogits(const void* H, int64_t ldh, const void* W, int64_t ldw, const int64_t* target,
+                          const float* lse, const float* grad_loss, void* D, int64_t ldd, int M, int K, int v_begin,
+                          int v_end, void* stream);
 
 #ifdef __cplusplus
 }
