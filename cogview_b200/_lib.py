@@ -22,19 +22,6 @@ class CogViewB200Error(RuntimeError):
     pass
 
 
-class DecodeStepArgs(ctypes.Structure):
-    """cv_decode_step_args of include/cogview_b200.h (host struct)."""
-    _fields_ = [("layers", c_void_p),
-                ("num_layers", c_int), ("hidden", c_int), ("heads", c_int), ("vocab", c_int), ("batch", c_int),
-                ("max_len", c_int),
-                ("eps", c_float), ("eps_final", c_float),
-                ("wte", c_void_p), ("wpe", c_void_p), ("lnf_g", c_void_p), ("lnf_b", c_void_p),
-                ("ids", c_void_p), ("pos", c_void_p), ("cur_len", c_void_p),
-                ("cache", c_void_p), ("cache_layer_stride", c_int64), ("cache_batch_stride", c_int64),
-                ("logits", c_void_p), ("ld_logits", c_int64),
-                ("workspace", c_void_p), ("prof", c_void_p)]
-
-
 def _declare(lib):
     lib.cv_version.restype = c_int
     lib.cv_last_error.restype = ctypes.c_char_p
@@ -93,7 +80,6 @@ def _declare(lib):
         "cv_attn_sparse_fwd_dropout": [P, L, L, P, L, L, P, L, L, P, P, L, L, P, P, I, I, I, I, I, I, I, F, U64, U32, P,
                                        P],
         "cv_attn_sparse_bwd_dropout": [P, L, L, P, L, L, P, L, L, P, P, P, P, P, P, I, I, I, I, I, I, I, F, P, P],
-        "cv_decode_step": [ctypes.POINTER(DecodeStepArgs), P],
         "cv_sample_topk": [P, L, I, I, F, I, ctypes.POINTER(c_int), I, U64, P, P, P, P, L, P, P, P, P, P, P],
         "cv_vocab_logprob": [P, L, P, L, P, P, P, I, I, I, I, P],
         "cv_vocab_xent_fwd": [P, L, P, L, P, P, P, P, I, I, I, P],
@@ -106,8 +92,6 @@ def _declare(lib):
     lib.cv_attn_sparse_bwd_workspace_bytes.restype = L
     lib.cv_attn_sparse_drop_mask_words.argtypes = [I, I, I, I, I, I]
     lib.cv_attn_sparse_drop_mask_words.restype = L
-    lib.cv_decode_step_workspace_bytes.argtypes = [I, I]
-    lib.cv_decode_step_workspace_bytes.restype = L
     lib.cv_layernorm_bwd_workspace_bytes.argtypes = [I, I]
     lib.cv_layernorm_bwd_workspace_bytes.restype = L
     lib.cv_attn_bwd_workspace_bytes.argtypes = [I, I, I, I]

@@ -582,18 +582,6 @@ extern "C" int cv_linear_small_m(const void* x, int64_t ldx, const void* W, int6
         cvh::count_launches(1);
         return 0;
     }
-    // COGVIEW_B200_LINEAR_RING=1: the bulk-copy-ring kernel (csrc/linear_ring.cu) for M <= 8.  Parity-green, opt-in:
-    // the decode step is bound by the latency of its ~340 dependent launches, not by the streaming rate of one of them.
-    static int use_ring = -1;
-    if (use_ring < 0) {
-        const char* e = getenv("COGVIEW_B200_LINEAR_RING");
-        use_ring = (e && e[0] == '1') ? 1 : 0;
-    }
-    if (use_ring) {
-        const int rc = cvh::linear_ring(xb, ldx, wb, ldw, bb, out, ldo, out_is_f32, act, absmax, M, N, K, s);
-        if (rc == 0) return 0;
-        if (rc != 1) return rc;
-    }
     CV_CUDA(cvh::launch_pdl(linear_small_m_kernel<SK_UNROLL, false>, dim3(grid), dim3(SK_WARPS * 32), 0, s, true, xb, ldx,
                             wb, ldw, bb, out, ldo, out_is_f32, act, absmax, M, N, K));
     cvh::count_launches(1);

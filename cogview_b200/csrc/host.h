@@ -76,11 +76,6 @@ cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t s
     return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 
-// csrc/linear_ring.cu: bulk-copy-ring variant of the small-M linear.  0 = launched, 1 = shape not handled here
-// (fall back to linear_small_m_kernel), anything else = error code.
-int linear_ring(const void* x, int64_t ldx, const void* W, int64_t ldw, const void* bias, void* out, int64_t ldo,
-                int out_is_f32, int act, float* absmax, int M, int N, int K, cudaStream_t s);
-
 enum class Swizzle { None, B128 };
 
 // Encode a tiled tensor map.  dims/strides are innermost-first, strides in BYTES for dims 1..rank-1.

@@ -206,8 +206,7 @@ def _generate_run_impl(self, last_tokens, first_pos, mems, n_steps, temperature,
     else:
         pos = torch.full((b, 1), int(first_pos), dtype=torch.long, device=last_tokens.device)
     # sparse inference: cv_sparse_plan is written for at most 16 sequences
-    if sparse is not None and (b > ops.DECODE_SMALL_MAX_BATCH or tr.max_memory_length > 4096 or runner.persistent
-                               or row_pad is not None):
+    if sparse is not None and (b > ops.DECODE_SMALL_MAX_BATCH or tr.max_memory_length > 4096 or row_pad is not None):
         return None
     new_tokens, logp = runner.sample_run(last_tokens.reshape(b, 1), pos, caches.t, n_steps, temperature, top_k,
                                          invalid_slices, sparse=sparse, row_pad=row_pad)

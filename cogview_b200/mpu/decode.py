@@ -3,18 +3,13 @@
 This is the fast path behind GPT2Model.forward when it is called the way generation/sampling.py:147-151 calls
 it (one new token per sequence, `mems` returned by the previous call, mems_mode 'kv').
 
-Two device paths:
-  * default: one kernel per operation (cv_attn_decode between cv_linear_small_m / cv_ln_pair_small_m at batch <= 16,
-    cv_linear_mid_m / cv_ln_pair_mid_m at batch 17..64), CUDA-graph captured; in generation runs followed by ONE
-    sampling kernel (cv_sample_topk) inside the same graph.  In ragged mode (rows from prompts of different lengths,
-    row_pad given) the attention is cv_attn_decode_ragged: row i holds cur_len - row_pad[i] cached tokens.  In shared
-    mode (a runner built on a kv_cache._SharedCaches: the beams of several prompts, each prompt's K|V held once) the
-    attention is cv_attn_decode_shared over the prompts' prefix cache and the rows' own suffix cache, and cur_len is
-    the suffix length.
-  * COGVIEW_B200_PERSISTENT=1 and batch <= 8: the whole step — embedding, 48 Sandwich-LN layers, final LayerNorm,
-    logits — is ONE persistent kernel (cv_decode_step, csrc/decode_step.cu: bulk-copy weight stream through a
-    shared-memory byte ring, register-resident residual stream, grid barriers between the dependency points).  Parity-
-    green and profiled per phase (tools/step_prof.py); it is opt-in, the per-operation path is the default.
+The step runs one kernel per operation (cv_attn_decode between cv_linear_small_m / cv_ln_pair_small_m at
+batch <= 16, cv_linear_mid_m / cv_ln_pair_mid_m at batch 17..64), CUDA-graph captured; in generation runs it is
+followed by ONE sampling kernel (cv_sample_topk) inside the same graph.  In ragged mode (rows from prompts of
+different lengths, row_pad given) the attention is cv_attn_decode_ragged: row i holds cur_len - row_pad[i] cached
+tokens.  In shared mode (a runner built on a kv_cache._SharedCaches: the beams of several prompts, each prompt's K|V
+held once) the attention is cv_attn_decode_shared over the prompts' prefix cache and the rows' own suffix cache, and
+cur_len is the suffix length.
 """
 import os
 
@@ -25,11 +20,9 @@ from .. import ops
 from .layers import _as_bf16
 
 
-def _persistent_enabled():
-    return os.environ.get('COGVIEW_B200_PERSISTENT', '0') == '1'
-
-
 class DecodeRunner:
+    persistent = False      # bench.py reads it; every step runs the per-operation kernels
+
     def __init__(self, model, caches, use_graph=True):
         tr = model.transformer
         self.model = model
@@ -54,8 +47,6 @@ class DecodeRunner:
         small = self.b <= ops.DECODE_SMALL_MAX_BATCH
         self.linear = ops.linear_small_m if small else ops.linear_mid_m
         self.ln_pair = ops.ln_pair_small_m if small else ops.ln_pair_mid_m
-        self.persistent = (_persistent_enabled() and self.b <= ops.DECODE_STEP_MAX_BATCH and self.h % 256 == 0
-                           and self.h <= 2560 and not self.shared)
         # enough (batch, head, split) CTAs to cover the SMs
         sms = torch.cuda.get_device_properties(dev).multi_processor_count
         # the key range of every (batch, head) is split so that ~8 CTAs per SM stream the K|V cache: the kernel is
@@ -95,12 +86,6 @@ class DecodeRunner:
                    _as_bf16(tr.final_layernorm.bias.detach()).contiguous(), tr.final_layernorm.eps)
         self.eps = tr.layers[0].layernorm_epsilon
         self.param_sig = self._signature()
-        dev = self.ids.device
-        if self.persistent:
-            table = torch.tensor([[t.data_ptr() for t in P] for P in self.params], dtype=torch.int64)
-            self.layer_table = table.to(dev)
-            self.workspace = ops.decode_step_workspace(self.h, self.heads, dev)
-            self.step_logits = torch.empty((self.b, self.wte.shape[0]), dtype=torch.float32, device=dev)
         # captured graphs hold the old pointers
         self.step_graphs = {}
         self.sample_graphs = {}
@@ -121,14 +106,6 @@ class DecodeRunner:
             self.len64 = torch.zeros((1, 1), dtype=torch.int64, device=dev)
 
     def _run(self):
-        if self.persistent and self.sparse is None and not self.ragged:
-            ops.decode_step(self.layer_table, len(self.params), self.heads, self.eps, self.fl[2], self.wte, self.wpe,
-                            self.fl[0], self.fl[1], self.ids, self.pos, self.cur_len, self.caches.buf,
-                            self.step_logits, self.workspace)
-            return self.step_logits
-        return self._run_per_op()
-
-    def _run_per_op(self):
         b, h, heads = self.b, self.h, self.heads
         L = len(self.params)
         scal = ops.new_scalars(2 * L + 1, self.ids.device)

@@ -612,39 +612,6 @@ LN_PAIR_MID_MAX_HIDDEN = 2560      # cv_ln_pair_mid_m keeps a row in the registe
 def decode_batch_supported(b, hidden):
     """True if the per-operation decode kernels cover b sequences per step at this hidden size."""
     return b <= DECODE_SMALL_MAX_BATCH or (b <= DECODE_MAX_BATCH and hidden <= LN_PAIR_MID_MAX_HIDDEN)
-DECODE_STEP_MAX_BATCH = 8
-
-
-def decode_step_workspace(hidden, heads, device):
-    """Zeroed workspace of the persistent decode step (counters + L2-resident activations)."""
-    n = lib().cv_decode_step_workspace_bytes(int(hidden), int(heads))
-    if n <= 0:
-        raise _lib.CogViewB200Error("cv_decode_step_workspace_bytes(%d, %d) failed" % (hidden, heads))
-    return torch.zeros(n, dtype=torch.uint8, device=device)
-
-
-def decode_step(layer_table, num_layers, heads, eps, eps_final, wte, wpe, lnf_g, lnf_b, ids, pos, cur_len, cache,
-                logits, workspace, prof=None):
-    """One token per sequence through every layer + logits in ONE kernel (cv_decode_step).
-    layer_table: int64 [num_layers, 16] device tensor of parameter pointers in cv_decode_layer order;
-    cache: [L, b, max_len, 2h] bf16; ids/pos: int64 [b(,1)]; cur_len: int32 [1]; logits: fp32 [b, V] (written)."""
-    require_cuda(layer_table, wte, wpe, lnf_g, lnf_b, ids, pos, cur_len, cache, logits, workspace)
-    L, b, max_len, h2 = cache.shape
-    assert L == num_layers and cache.dtype == torch.bfloat16 and cache.stride(3) == 1 and cache.stride(2) == h2
-    assert layer_table.dtype == torch.int64 and layer_table.shape == (num_layers, 16) and layer_table.is_contiguous()
-    assert ids.dtype == torch.int64 and pos.dtype == torch.int64 and ids.numel() == b and pos.numel() == b
-    assert ids.is_contiguous() and pos.is_contiguous() and cur_len.dtype == torch.int32
-    assert logits.dtype == torch.float32 and logits.shape[0] == b and logits.stride(1) == 1
-    assert wte.dtype == torch.bfloat16 and wte.is_contiguous() and wpe.is_contiguous()
-    a = _lib.DecodeStepArgs(
-        layers=ptr(layer_table), num_layers=num_layers, hidden=h2 // 2, heads=heads, vocab=wte.shape[0], batch=b,
-        max_len=max_len, eps=float(eps), eps_final=float(eps_final), wte=ptr(wte), wpe=ptr(wpe), lnf_g=ptr(lnf_g),
-        lnf_b=ptr(lnf_b), ids=ptr(ids), pos=ptr(pos), cur_len=ptr(cur_len), cache=ptr(cache),
-        cache_layer_stride=cache.stride(0), cache_batch_stride=cache.stride(1), logits=ptr(logits),
-        ld_logits=logits.stride(0), workspace=ptr(workspace), prof=ptr(prof))
-    import ctypes
-    check(lib().cv_decode_step(ctypes.byref(a), stream_ptr()), "cv_decode_step")
-    return logits
 
 
 def valid_ranges(invalid, vocab):

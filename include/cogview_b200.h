@@ -295,48 +295,6 @@ int cv_attn_decode_gather(const void* qkv, void* cache, int64_t cache_batch_stri
                           int head_dim, int max_len, int nsplit, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Whole decode step as ONE persistent kernel (1 <= batch <= 8): what GPT2Model.forward (model/gpt2_modeling.py:106-123)
- * computes when generation/sampling.py:147-151 calls it with one new token per sequence — embedding, every
- * Sandwich-LN layer (mpu/sparse_transformer.py:314-342: LN1, QKV, attention over the K|V cache + append, dense,
- * x + LN3, LN2, h->4h + GELU, 4h->h, y + LN4), final LayerNorm and the tied-embedding logits.  One CTA per SM
- * stays resident; a producer warp streams each CTA's share of every weight matrix through a shared-memory ring
- * with cp.async.bulk (the stream runs ahead across the grid barriers of a layer), consumer warps feed mma.sync
- * from shared memory; csrc/decode_step.cu has the design.
- *   layers: DEVICE array of cv_decode_layer structs: bf16 tensors, reference parameter shapes, weights [out, in].
- *   cache: [num_layers, batch, max_len, 2*hidden] bf16 (K | V), strides in elements; the new token is appended at
- *     *cur_len.  ids / pos: int64 [batch].  logits: fp32 [batch, ld_logits].
- *   workspace: cv_decode_step_workspace_bytes(hidden, heads) bytes, 256-byte aligned, ZEROED once by the caller
- *     (it holds the grid-barrier and arrival counters, which the kernel leaves consistent for the next call).
- * ---------------------------------------------------------------------------------------------- */
-typedef struct cv_decode_layer {
-    const void *ln1_g, *ln1_b;       /* input_layernorm                       [h]      */
-    const void *w_qkv, *b_qkv;       /* attention.query_key_value             [3h, h]  */
-    const void *w_dense, *b_dense;   /* attention.dense                       [h, h]   */
-    const void *ln3_g, *ln3_b;       /* third_layernorm                                */
-    const void *ln2_g, *ln2_b;       /* post_attention_layernorm                       */
-    const void *w_fc1, *b_fc1;       /* mlp.dense_h_to_4h                     [4h, h]  */
-    const void *w_fc2, *b_fc2;       /* mlp.dense_4h_to_h                     [h, 4h]  */
-    const void *ln4_g, *ln4_b;       /* fourth_layernorm                               */
-} cv_decode_layer;                   /* 128 bytes */
-typedef struct cv_decode_step_args {
-    const cv_decode_layer* layers;
-    int num_layers, hidden, heads, vocab, batch, max_len;
-    float eps, eps_final;
-    const void *wte, *wpe, *lnf_g, *lnf_b;
-    const int64_t *ids, *pos;
-    const int* cur_len;
-    void* cache;
-    int64_t cache_layer_stride, cache_batch_stride;
-    float* logits;
-    int64_t ld_logits;
-    void* workspace;
-    void* prof;   /* NULL, or uint64 [SMs][num_layers][32]: %globaltimer stamps of the 13 phase boundaries of every
-                     layer and wait-cycle accounting of the four linears, per CTA (tools/step_prof.py) */
-} cv_decode_step_args;               /* HOST struct */
-int64_t cv_decode_step_workspace_bytes(int hidden, int heads);
-int cv_decode_step(const cv_decode_step_args* args, void* stream);
-
-/* ------------------------------------------------------------------------------------------------
  * Sampling epilogue of the decode loop in one kernel (one CTA per sequence): generation/sampling.py:157-183 with
  * top_k_logits (:24-33) — logits / temperature, invalid vocabulary slices, keep every logit >= the k-th largest
  * (exact radix select; ties at the threshold are all kept, as `logits < kth` does), softmax over the kept ones,

@@ -4,8 +4,9 @@ DecodeRunner built on them, generation with 32 beams and the post-selection driv
 Tolerances: the linear against an fp32 product of the same bf16 inputs — 1e-4 of the row scale for fp32 outputs
 (summation order only), 2e-2 for bf16 outputs (rounding of the result); the LayerNorm pair against the 8-row
 instance of cv_ln_pair_small_m given the same abs-max scalars — the residual stream y to 1e-6 of its scale, xn to one
-bf16 step (same arithmetic, same reduction order) — and against the fp64 oracle; the decode step
-with the bounds of test_decode_step_gpu.py::test_persistent_step_matches_per_op_path.
+bf16 step (same arithmetic, same reduction order) — and against the fp64 oracle; the graph-replayed decode step
+against the general GEMM route of GPT2Model.forward — logits within 1e-2 of the logit scale (bf16 paths that differ
+in summation order), the appended K|V rows within bf16 rounding, older cache rows untouched.
 """
 import pytest
 import torch
@@ -118,6 +119,9 @@ def test_ln_pair_mid_m(ops, M, K):
 # ----------------------------------------------------------------------------------------------------
 CFG_TINY = dict(num_layers=2, vocab_size=58240, hidden_size=256, num_attention_heads=4)
 CFG_WIDE = dict(num_layers=2, vocab_size=8192 + 512, hidden_size=2560, num_attention_heads=40)
+CFG_MID = dict(num_layers=3, vocab_size=4096, hidden_size=1024, num_attention_heads=16)
+CFG_512 = dict(num_layers=2, vocab_size=1000, hidden_size=512, num_attention_heads=8)
+CFG_768 = dict(num_layers=2, vocab_size=1000, hidden_size=768, num_attention_heads=12)
 
 
 def _model(cfg, maxlen, seed=7):
@@ -134,10 +138,14 @@ def _model(cfg, maxlen, seed=7):
 
 
 @pytest.mark.parametrize("cfg,b,t", [(CFG_TINY, 17, 0), (CFG_TINY, 32, 127), (CFG_TINY, 64, 1085), (CFG_TINY, 64, 0),
-                                     (CFG_WIDE, 17, 127), (CFG_WIDE, 32, 0), (CFG_WIDE, 32, 1085), (CFG_WIDE, 64, 127)])
+                                     (CFG_WIDE, 17, 127), (CFG_WIDE, 32, 0), (CFG_WIDE, 32, 1085), (CFG_WIDE, 64, 127),
+                                     (CFG_TINY, 1, 0), (CFG_TINY, 3, 17), (CFG_TINY, 4, 120), (CFG_TINY, 8, 64),
+                                     (CFG_MID, 2, 33), (CFG_MID, 5, 250), (CFG_512, 4, 40), (CFG_768, 6, 77),
+                                     (CFG_WIDE, 4, 0), (CFG_WIDE, 4, 300), (CFG_WIDE, 7, 129), (CFG_WIDE, 8, 1085)])
 def test_graph_step_matches_the_general_route(cfg, b, t, monkeypatch):
-    """The replayed graph of the mid-batch kernels against GPT2Model.forward with the fast path switched off
-    (training GEMM tiles, cv_attn_fwd with one query) on the same weights and cache."""
+    """The replayed graph of the decode kernels (the small-M pair up to 16 sequences, the mid-batch pair above)
+    against GPT2Model.forward with the fast path switched off (training GEMM tiles, cv_attn_fwd with one query) on
+    the same weights and cache."""
     from cogview_b200.mpu import kv_cache
     from cogview_b200.mpu.decode import DecodeRunner
     maxlen = 1089 if t > 200 else 256
@@ -149,7 +157,8 @@ def test_graph_step_matches_the_general_route(cfg, b, t, monkeypatch):
     c.buf.copy_(base)
     c.t = t
     r = DecodeRunner(model, c, use_graph=True)
-    assert r.linear.__name__ == "linear_mid_m" and r.ln_pair.__name__ == "ln_pair_mid_m" and not r.persistent
+    kind = "small_m" if b <= 16 else "mid_m"
+    assert r.linear.__name__ == "linear_" + kind and r.ln_pair.__name__ == "ln_pair_" + kind
     monkeypatch.setenv("COGVIEW_B200_FAST_DECODE", "0")
     mems = [base[i, :, :t].clone() for i in range(cfg["num_layers"])] + [base.new_empty((b, t, 0))] if t > 0 else []
     ids = torch.randint(0, cfg["vocab_size"], (b, 1), generator=torch.Generator().manual_seed(t)).cuda()

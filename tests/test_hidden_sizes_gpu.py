@@ -6,8 +6,7 @@ The library picks kernels by hidden size in several places:
     kernel otherwise (csrc/layernorm.cu cv_layernorm_absmax_fwd);
   * LayerNorm backward: the fused kernel for cols % 256 == 0 and cols <= 4096, else ln_bwd_dx_kernel +
     ln_bwd_param_kernel + ln_bwd_finalize_kernel;
-  * layer backward: bias gradients from the fused LayerNorm backward's column sums, or from cv_colsum_bf16;
-  * decode: the persistent step only for h % 256 == 0 and h <= 2560, the per-operation graph otherwise.
+  * layer backward: bias gradients from the fused LayerNorm backward's column sums, or from cv_colsum_bf16.
 
 Errors are checked per row (per 128 x 128 block for GEMM outputs) against that row's (block's) scale, so a wrong tail
 row or tile cannot hide behind a large value elsewhere.  Tolerances as in test_kernels_gpu.py: 2e-2 of the scale for
@@ -440,12 +439,9 @@ def test_output_dropout_at_h384_matches_oracle(monkeypatch):
 # ----------------------------------------------------------------------------------------------------
 # decode off the grid
 # ----------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("persistent_requested", [False, True])
-def test_kv_decode_at_h320_matches_full_prefix_forward(monkeypatch, persistent_requested):
+def test_kv_decode_at_h320_matches_full_prefix_forward(monkeypatch):
     """Prefill 64 tokens, then 16 single-token steps through the K|V-cache decode graph; each step's logits against a
-    no-memory forward over the whole prefix with the same weights.  The persistent step does not take h = 320, so
-    asking for it must leave the per-operation path in place."""
-    monkeypatch.setenv("COGVIEW_B200_PERSISTENT", "1" if persistent_requested else "0")
+    no-memory forward over the whole prefix with the same weights."""
     monkeypatch.setenv("COGVIEW_B200_CUDA_GRAPH", "1")
     h, heads, b, n0, n = 320, 5, 2, 64, 16
     m, _ = _gpt2(h, heads, 2, 128, max_mem=128)
@@ -468,7 +464,6 @@ def test_kv_decode_at_h320_matches_full_prefix_forward(monkeypatch, persistent_r
             assert e < 2e-2, (t, e)
     runner = m.transformer._kv.runner
     print("h=320 decode: worst step logits error / row scale %.3e, graph replays %d" % (worst, runner.replays))
-    assert runner.persistent is False
     assert runner.replays == n
 
 

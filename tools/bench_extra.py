@@ -1,8 +1,8 @@
 """Measurements that are claimed in DESIGN.md but are not part of bench.py's headline line:
 
-  sweep     : SURVEY §8(d) config 2 batch sweep — AR sampling tokens/s of the 4B model at b = 1, 4, 8 (persistent
-              one-kernel step), 16 (per-operation decode kernels, cv_linear_small_m M <= 16) and 64 (per-operation
-              decode kernels, cv_linear_mid_m 17 <= M <= 64); tools/decode_batch_time.py times the routes side by side
+  sweep     : SURVEY §8(d) config 2 batch sweep — AR sampling tokens/s of the 4B model at b = 1, 4, 8, 16
+              (per-operation decode kernels, cv_linear_small_m M <= 16) and 64 (per-operation decode kernels,
+              cv_linear_mid_m 17 <= M <= 64); tools/decode_batch_time.py times the routes side by side
   sr_dense  : BASELINE configs[4] as the reference SHIPS it (scripts/super_resolution.sh:7,36): dense attention,
               1345 positions — context 321 tokens, 1024 generated, 4 beams
   sr_sparse : BASELINE configs[4] as the config names it: is_sparse = 2 (sparse_attention_inference,
@@ -52,8 +52,7 @@ def main():
         for b in [int(x) for x in a.batches.split(",")]:
             seq = bench.make_template(b, a.gen, seed=0).cuda()
             ms, out = timed_fill(model, seq, bench.SampleArgs)
-            path = "persistent one-kernel step" if b <= 8 else ("per-operation decode kernels" if b <= 64
-                                                                else "general GEMM path + K|V cache")
+            path = "per-operation decode kernels" if b <= 64 else "general GEMM path + K|V cache"
             out_lines.append(dict(workload="batch sweep", batch=b, gen_tokens=a.gen, ms=ms, tokens_per_s=b * a.gen / ms * 1e3,
                                   ms_per_token_step=ms / a.gen, path=path))
             print(json.dumps(out_lines[-1]), flush=True)

@@ -1,7 +1,7 @@
 """The four decode linears of a 4B layer (M = 4) back to back, CUDA-graph replayed like the decode step (PDL between
 them), L2 flushed by the 157 MB of weights themselves: us per layer-set and achieved HBM bandwidth.
 
-    python tools/linear_time.py             (COGVIEW_B200_LINEAR_RING=1 selects the bulk-copy-ring kernel)"""
+    python tools/linear_time.py"""
 import os
 import sys
 
