@@ -111,14 +111,19 @@ def load_checkpoint(model, optimizer=None, lr_scheduler=None, load_dir=None, *, 
 
 def save_checkpoint(iteration, model, optimizer, lr_scheduler, save_dir, *, no_save_optim=False, no_save_rng=False,
                     release=False, rank=0):
-    """utils.py:188-232: rank 0 of the data-parallel group writes the file and the tracker."""
+    """utils.py:188-232: rank 0 of the data-parallel group writes the file and the tracker.  A sharded optimizer
+    (optim.ShardedFusedAdamW) is saved in FusedAdamW's form through its consolidated_state_dict(), which every rank
+    takes part in: call this function on every rank then."""
+    osd = None
+    if not no_save_optim and optimizer is not None and hasattr(optimizer, 'consolidated_state_dict'):
+        osd = optimizer.consolidated_state_dict()
     if rank != 0:
         return None
     name = get_checkpoint_name(save_dir, iteration, release)
     sd = {'iteration': iteration, 'module': _unwrap(model).state_dict()}
     if not no_save_optim:
         if optimizer is not None:
-            sd['optimizer'] = optimizer.state_dict()
+            sd['optimizer'] = osd if osd is not None else optimizer.state_dict()
         if lr_scheduler is not None:
             sd['lr_scheduler'] = lr_scheduler.state_dict()
     if not no_save_rng:

@@ -65,7 +65,8 @@ def train_step(batch, model, optimizer, lr_scheduler=None, txt_loss_scale=1.0, i
         return partial, 1, mems, img_loss, txt_loss
     optimizer.zero_grad(set_to_none=True)
     lm_loss.backward()                    # torch DDP averages the gradients over the data-parallel group here
-    optimizer.step()                      # FusedAdamW: global-norm clip + AdamW, no host sync
+    optimizer.step()                      # FusedAdamW: global-norm clip + AdamW, no host sync (ShardedFusedAdamW:
+    #                                       reduce-scatter of the gradients, clip + AdamW on the shard, all-gather)
     # an inf / NaN gradient norm makes FusedAdamW leave every tensor untouched (fp16/fp16.py:399-420, the overflow
     # branch of FP16_Optimizer.step): report it like the reference does and do not advance the schedule
     flag = getattr(optimizer, 'last_step_skipped', None)
