@@ -83,14 +83,28 @@ def get_tokenizer(args=None):
 
 # ----------------------------------------------------------------------------------------------------
 def get_masks_and_position_ids(data, loss_mask=None, attention_mask=None, args=None):
-    """pretrain_gpt2.py:210-253 (pre-training branch): lower-triangular [1,1,s,s] mask, ones loss mask, arange
-    position ids."""
+    """pretrain_gpt2.py:210-253: lower-triangular [1,1,s,s] mask, ones loss mask, arange position ids.
+
+    With `args.finetune` and args.max_position_embeddings < args.max_position_embeddings_finetune (the finetune
+    branch, :228-247: two-image rows longer than the position table), each row's positions restart at 0 at its
+    first [ROI2], which takes position 0 itself, and every position >= max_position_embeddings is then clamped to
+    max_position_embeddings - 1.  Computed on the device in one pass (the reference loops over the rows in Python);
+    a row without [ROI2] raises AssertionError('Some samples do not have [ROI2]!'), which reads one flag to the host.
+    Sampling (filling_sequence) gives the tokens after [ROI2] the same positions 1, 2, ... but keeps [ROI2] itself at
+    its own index; that mismatch is the reference's, and this branch keeps its training positions."""
     batch_size, seq_length = data.size()
     if attention_mask is None:
         attention_mask = torch.tril(torch.ones((1, seq_length, seq_length), device=data.device)).unsqueeze(1)
     if loss_mask is None:
         loss_mask = torch.ones(data.size(), dtype=torch.float, device=data.device)
-    position_ids = torch.arange(seq_length, dtype=torch.long, device=data.device).unsqueeze(0).expand_as(data)
+    if (args is not None and getattr(args, 'finetune', False)
+            and args.max_position_embeddings < args.max_position_embeddings_finetune):
+        ar = torch.arange(seq_length, dtype=torch.long, device=data.device).unsqueeze(0)
+        first = torch.where(data == get_tokenizer()['[ROI2]'], ar, seq_length).amin(dim=1, keepdim=True)
+        assert bool((first < seq_length).all()), 'Some samples do not have [ROI2]!'
+        position_ids = torch.where(ar < first, ar, ar - first).clamp_max(args.max_position_embeddings - 1)
+    else:
+        position_ids = torch.arange(seq_length, dtype=torch.long, device=data.device).unsqueeze(0).expand_as(data)
     return attention_mask, loss_mask, position_ids
 
 
