@@ -81,6 +81,7 @@ def _declare(lib):
                                        P],
         "cv_attn_sparse_bwd_dropout": [P, L, L, P, L, L, P, L, L, P, P, P, P, P, P, I, I, I, I, I, I, I, F, P, P],
         "cv_sample_topk": [P, L, I, I, F, I, ctypes.POINTER(c_int), I, U64, P, P, P, P, L, P, P, P, P, P, P],
+        "cv_sample_topk_topp": [P, L, I, I, F, I, ctypes.POINTER(c_int), I, U64, P, P, P, P, L, P, P, P, P, P, F, P],
         "cv_vocab_logprob": [P, L, P, L, P, P, P, I, I, I, I, P],
         "cv_vocab_xent_fwd": [P, L, P, L, P, P, P, P, I, I, I, P],
         "cv_vocab_xent_dlogits": [P, L, P, L, P, P, P, P, L, I, I, I, I, P],

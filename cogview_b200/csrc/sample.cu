@@ -4,6 +4,17 @@
 // Reference: generation/sampling.py:157-183 and top_k_logits :24-33 (`logits[logits < kth] = -inf`: every logit equal
 // to the k-th largest survives).  The k-th largest value is found exactly with a 4-pass radix select on the
 // order-preserving integer image of the floats; the row (<= 233 KB, 32 KB for image tokens) stays in L1/L2.
+//
+// Nucleus (top-p) filtering, top_k_logits :34-47, is the NUCLEUS instantiation: applied after top-k, over the
+// softmax of the top-k survivors.  The reference sorts descending, takes the cumulative sum and shifts it by one, so
+// a token survives iff the probability mass strictly above it is <= top_p (the first token that takes the mass past
+// top_p is kept).  The boundary key is found with a second 4-pass radix descent on the same keys whose histograms
+// hold probability MASS per bin: exp(x - max) in 2^-40 fixed point (<= 2^56 over 58240 entries), summed first over
+// the lanes of a warp that share a bin, then with exact integer shared-memory atomics, so the sums do not depend on
+// the order of the adds and every call is bit-reproducible.  Every token
+// whose logit equals the boundary logit is kept (the same rule as top-k's `logits < kth`); torch.sort leaves the
+// order among ties unspecified, so the reference has no defined answer there.  top_p >= 1, or a mass that is never
+// exceeded, keeps every top-k survivor.
 #include "common.cuh"
 #include "host.h"
 #include "../../include/cogview_b200.h"
@@ -38,7 +49,8 @@ __device__ __forceinline__ uint32_t f2key(float f) {
     return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 
-__global__ void __launch_bounds__(ST) sample_topk_kernel(const SampleParams p) {
+template <bool NUCLEUS>
+__global__ void __launch_bounds__(ST) sample_topk_kernel(const SampleParams p, const float top_p) {
     __shared__ int hist[256];
     __shared__ float wred[SW];
     __shared__ float wcum[SW];
@@ -127,6 +139,94 @@ __global__ void __launch_bounds__(ST) sample_topk_kernel(const SampleParams p) {
             __syncthreads();
         }
         thr = s_prefix;
+    }
+
+    if constexpr (NUCLEUS) {
+        // ---- nucleus boundary: the largest key whose mass strictly above is > limit ends the kept set ----------
+        // The mass of a bin is kept as three 16-bit digits in 32-bit counters: every add is < 2^16 per digit and a
+        // bin gets at most 58240 adds, so the counters never wrap, and 32-bit shared atomics are native (a 64-bit
+        // shared add is a compare-and-swap loop, which the few hot bins of the first pass would serialise on).
+        __shared__ unsigned int mhist[3][256];
+        __shared__ unsigned long long s_above;          // mass of the kept keys above the current prefix
+        __shared__ uint32_t s_pprefix;
+        __shared__ int s_all;
+        auto bin_mass = [&](int bin) -> unsigned long long {
+            return (unsigned long long)mhist[0][bin] + ((unsigned long long)mhist[1][bin] << 16) +
+                   ((unsigned long long)mhist[2][bin] << 32);
+        };
+        if (top_p < 1.f) {
+            if (tid == 0) { s_pprefix = 0; s_above = 0; s_all = 0; }
+            unsigned long long limit = 0;                   // floor(top_p * total), warp 0 only
+            uint32_t himask = 0;
+            for (int shift = 24; shift >= 0; shift -= 8) {
+                if (tid < 256) mhist[0][tid] = mhist[1][tid] = mhist[2][tid] = 0u;
+                __syncthreads();
+                const uint32_t prefix = s_pprefix;
+                for (int it = 0; it < nit; ++it) {
+                    const int i = warp * R + it * 32 + lane;
+                    unsigned int bin = 256u;                // 256: this lane adds nothing
+                    unsigned long long w = 0;               // exp(x - max) * 2^40 <= 2^40
+                    if (i < p.nvalid) {
+                        const float x = value(real_index(i));
+                        const uint32_t key = f2key(x);
+                        if (key >= thr && ((key ^ prefix) & himask) == 0) {
+                            bin = (key >> shift) & 255u;
+                            w = __float2ull_rz(__expf(x - mx) * 0x1p40f);
+                        }
+                    }
+                    if (__any_sync(0xffffffffu, bin < 256u)) {
+                        // one add per distinct bin of the warp: the lanes of a bin sum their 20-bit halves
+                        const unsigned int peers = __match_any_sync(0xffffffffu, bin);
+                        const unsigned int lo = __reduce_add_sync(peers, (unsigned int)(w & 0xfffffu));
+                        const unsigned int hi = __reduce_add_sync(peers, (unsigned int)(w >> 20));
+                        if (bin < 256u && lane == __ffs(peers) - 1) {
+                            const unsigned long long s = ((unsigned long long)hi << 20) + lo;     // <= 2^45
+                            atomicAdd(&mhist[0][bin], (unsigned int)(s & 0xffffu));
+                            atomicAdd(&mhist[1][bin], (unsigned int)((s >> 16) & 0xffffu));
+                            atomicAdd(&mhist[2][bin], (unsigned int)(s >> 32));
+                        }
+                    }
+                }
+                __syncthreads();
+                if (warp == 0) {
+                    // lane L owns bins 255-8L .. 248-8L (descending); find the bin where the mass from the top
+                    // passes the limit
+                    unsigned long long c = 0;
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) c += bin_mass(255 - 8 * lane - j);
+                    unsigned long long cum = c;
+#pragma unroll
+                    for (int o = 1; o < 32; o <<= 1) {
+                        const unsigned long long t = __shfl_up_sync(0xffffffffu, cum, o);
+                        if (lane >= o) cum += t;
+                    }
+                    if (shift == 24)                        // the first pass holds every kept entry
+                        limit = (unsigned long long)((double)top_p * (double)__shfl_sync(0xffffffffu, cum, 31));
+                    const unsigned long long above = s_above;
+                    const unsigned int bal = __ballot_sync(0xffffffffu, above + cum > limit);
+                    const int sel = __ffs(bal) - 1;
+                    if (bal == 0) {                         // first pass only: the mass never exceeds top_p
+                        if (lane == 0) s_all = 1;
+                    } else if (lane == sel) {
+                        unsigned long long before = above + cum - c;
+                        for (int j = 0; j < 8; ++j) {
+                            const int bin = 255 - 8 * lane - j;
+                            const unsigned long long m = bin_mass(bin);
+                            if (before + m > limit) {
+                                s_pprefix = prefix | ((uint32_t)bin << shift);
+                                s_above = before;
+                                break;
+                            }
+                            before += m;
+                        }
+                    }
+                }
+                himask |= 0xffu << shift;
+                __syncthreads();
+                if (s_all) break;
+            }
+            if (!s_all) thr = max(thr, s_pprefix);
+        }
     }
 
     // ---- softmax denominator over the kept entries, in (warp, iteration, lane) order ---------------
@@ -227,13 +327,10 @@ __global__ void __launch_bounds__(ST) sample_topk_kernel(const SampleParams p) {
     }
 }
 
-}  // namespace
-
-extern "C" int cv_sample_topk(const float* logits, int64_t ld, int b, int vocab, float temperature, int top_k,
-                              const int* valid, int n_valid, uint64_t seed, const uint64_t* seed_dev, int64_t* step,
-                              int64_t* next_ids,
-                              int64_t* out_tokens, int64_t ld_out, float* score_acc, int64_t* pos, int* cur_len,
-                              unsigned int* done_counter, float* probs_out, void* stream) {
+int launch_sample(const float* logits, int64_t ld, int b, int vocab, float temperature, int top_k, const int* valid,
+                  int n_valid, uint64_t seed, const uint64_t* seed_dev, int64_t* step, int64_t* next_ids,
+                  int64_t* out_tokens, int64_t ld_out, float* score_acc, int64_t* pos, int* cur_len,
+                  unsigned int* done_counter, float* probs_out, void* stream, bool nucleus, float top_p) {
     CV_REQUIRE(logits && next_ids && valid, "null pointer");
     CV_REQUIRE(b >= 1 && vocab >= 1 && ld >= vocab, "bad sizes");
     CV_REQUIRE(n_valid >= 1 && n_valid <= 4, "1..4 valid vocabulary ranges");
@@ -256,7 +353,29 @@ extern "C" int cv_sample_topk(const float* logits, int64_t ld, int b, int vocab,
     p.nvalid = total;
     p.seed = seed; p.seed_dev = seed_dev; p.step = step; p.next_ids = next_ids; p.out_tokens = out_tokens; p.ld_out = ld_out;
     p.score_acc = score_acc; p.pos = pos; p.cur_len = cur_len; p.done = done_counter; p.probs_out = probs_out;
-    sample_topk_kernel<<<b, ST, 0, static_cast<cudaStream_t>(stream)>>>(p);
+    if (nucleus) sample_topk_kernel<true><<<b, ST, 0, static_cast<cudaStream_t>(stream)>>>(p, top_p);
+    else sample_topk_kernel<false><<<b, ST, 0, static_cast<cudaStream_t>(stream)>>>(p, 0.f);
     CV_LAUNCH_CHECK();
     return 0;
+}
+
+}  // namespace
+
+extern "C" int cv_sample_topk(const float* logits, int64_t ld, int b, int vocab, float temperature, int top_k,
+                              const int* valid, int n_valid, uint64_t seed, const uint64_t* seed_dev, int64_t* step,
+                              int64_t* next_ids,
+                              int64_t* out_tokens, int64_t ld_out, float* score_acc, int64_t* pos, int* cur_len,
+                              unsigned int* done_counter, float* probs_out, void* stream) {
+    return launch_sample(logits, ld, b, vocab, temperature, top_k, valid, n_valid, seed, seed_dev, step, next_ids,
+                         out_tokens, ld_out, score_acc, pos, cur_len, done_counter, probs_out, stream, false, 0.f);
+}
+
+extern "C" int cv_sample_topk_topp(const float* logits, int64_t ld, int b, int vocab, float temperature, int top_k,
+                                   const int* valid, int n_valid, uint64_t seed, const uint64_t* seed_dev,
+                                   int64_t* step, int64_t* next_ids, int64_t* out_tokens, int64_t ld_out,
+                                   float* score_acc, int64_t* pos, int* cur_len, unsigned int* done_counter,
+                                   float* probs_out, float top_p, void* stream) {
+    CV_REQUIRE(top_p > 0.f, "top_p must be positive (cv_sample_topk samples without the nucleus)");
+    return launch_sample(logits, ld, b, vocab, temperature, top_k, valid, n_valid, seed, seed_dev, step, next_ids,
+                         out_tokens, ld_out, score_acc, pos, cur_len, done_counter, probs_out, stream, true, top_p);
 }

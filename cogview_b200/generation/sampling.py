@@ -108,11 +108,27 @@ def get_masks_and_position_ids(data, loss_mask=None, attention_mask=None, args=N
     return attention_mask, loss_mask, position_ids
 
 
+def top_p_logits(logits, top_p, filter_value=-float('Inf')):
+    """The nucleus (top-p) filter of top_k_logits (generation/sampling.py:34-47) row by row on [b, V] logits, in
+    place: sort each row descending, take the cumulative softmax, shift it by one, and set every logit whose mass
+    before it in that order exceeds top_p to filter_value.  Sort, cumsum, a shift and a scatter only, no boolean
+    indexing, so it can be captured in a CUDA graph.  Each row gets what the reference's one-row branch gives it."""
+    sorted_logits, sorted_indices = torch.sort(logits, descending=True)
+    cumulative_probs = torch.cumsum(F.softmax(sorted_logits, dim=-1), dim=-1)
+    remove = cumulative_probs > top_p
+    remove[..., 1:] = remove[..., :-1].clone()
+    remove[..., 0] = False
+    return logits.masked_fill_(torch.zeros_like(remove).scatter_(-1, sorted_indices, remove), filter_value)
+
+
 def top_k_logits(logits, top_k=0, top_p=0.0, filter_value=-float('Inf')):
-    """generation/sampling.py:24-49."""
+    """generation/sampling.py:24-49.  The reference's top-p branch views the logits as one row; logits with more
+    than one row go through top_p_logits, which applies it to each row."""
     if top_k > 0:
         kth = torch.topk(logits, top_k)[0][..., -1, None]
         logits[logits < kth] = filter_value
+    if top_p > 0.0 and logits.dim() == 2 and logits.shape[0] > 1:
+        return top_p_logits(logits, top_p, filter_value)
     if top_p > 0.0:
         logits = logits.view(logits.size()[1]).contiguous()
         sorted_logits, sorted_indices = torch.sort(logits, descending=True)
@@ -253,12 +269,15 @@ def filling_sequence(model, seq, args, mems=None, invalid_slices=[], **kwargs):
                 run += 1
             first_pos = counter - offset if counter > offset else counter
             device_pivots = is_sparse == 2 and _os.environ.get('COGVIEW_B200_SPARSE_PIVOTS', 'device') != 'host'
-            if (run >= 2 and index == counter and tokens.shape[0] == -nxt and args.top_p == 0.0
+            # nucleus sampling of a single row keeps the host loop (and torch.multinomial's draws)
+            if (run >= 2 and index == counter and tokens.shape[0] == -nxt
+                    and (args.top_p == 0.0 or tokens.shape[0] > 1)
                     and (is_sparse == 0 or device_pivots)
                     and not (counter <= offset < counter + run) and hasattr(model, 'generate_run')):
                 sparse = dict(n_img=n_img, tokens=tokens) if is_sparse == 2 else None
+                nucleus = dict(top_p=args.top_p) if args.top_p > 0.0 else {}
                 res = model.generate_run(tokens[:, counter:], first_pos, mems, run, args.temperature, args.top_k,
-                                         invalid_slices, sparse=sparse)
+                                         invalid_slices, sparse=sparse, **nucleus)
                 if res is not None:
                     new_tokens, logp, mems = res
                     if -nxt > 1:

@@ -174,7 +174,7 @@ GPT2Model._fast_decode = _fast_decode_impl
 
 
 def _generate_run_impl(self, last_tokens, first_pos, mems, n_steps, temperature, top_k, invalid_slices, sparse=None,
-                       row_pad=None):
+                       row_pad=None, top_p=0.0):
     """n_steps sampled tokens in a row on the K|V cache — the inner loop of generation/sampling.py:147-183 for a
     stretch of the template that is all 'generate' slots — with the sampling tail inside the replayed CUDA graph
     (mpu/decode.py sample_run).  Returns None when the fast path does not apply, else
@@ -184,7 +184,8 @@ def _generate_run_impl(self, last_tokens, first_pos, mems, n_steps, temperature,
     token, chosen on the device (cv_sparse_plan) instead of Python's random.sample — same distribution, other stream.
     first_pos is one position for every row, or one per row (a sequence or 1-D tensor of b positions).
     row_pad (int32 [b] on the device, from mpu/kv_cache.py assemble): row i of `mems` holds mems[0].size(1) - row_pad[i]
-    tokens — rows of prompts of different lengths in one run (not with sparse)."""
+    tokens — rows of prompts of different lengths in one run (not with sparse).
+    top_p > 0 adds nucleus filtering after top-k (generation/sampling.py:34-47) to the sampling tail."""
     tr = self.transformer
     b = last_tokens.shape[0]
     if (not mems or tr.mems_mode != 'kv' or tr.max_memory_length <= 0 or torch.is_grad_enabled()
@@ -209,7 +210,7 @@ def _generate_run_impl(self, last_tokens, first_pos, mems, n_steps, temperature,
     if sparse is not None and (b > ops.DECODE_SMALL_MAX_BATCH or tr.max_memory_length > 4096 or row_pad is not None):
         return None
     new_tokens, logp = runner.sample_run(last_tokens.reshape(b, 1), pos, caches.t, n_steps, temperature, top_k,
-                                         invalid_slices, sparse=sparse, row_pad=row_pad)
+                                         invalid_slices, sparse=sparse, row_pad=row_pad, top_p=top_p)
     return new_tokens, logp, caches.views()
 
 

@@ -17,6 +17,7 @@ import torch
 import torch.nn.functional as F
 
 from .. import ops
+from ..generation.sampling import top_p_logits
 from .layers import _as_bf16
 
 
@@ -204,11 +205,12 @@ class DecodeRunner:
     # -- generation runs: generation/sampling.py:147-183 with nothing left on the host per token -----------------
     def _sample_body(self, key):
         """One token: decode step, then the reference's sampling tail — temperature, invalid vocabulary slices,
-        top-k (generation/sampling.py:24-33), softmax, multinomial draw, beam log-probability — and the hand-over of
-        the sampled token to the next step, all through device-side state.  With the fused kernel the tail is ONE
-        launch (cv_sample_topk, own counter-based generator); COGVIEW_B200_FUSED_SAMPLING=0 keeps the reference's
-        torch operations (torch.multinomial's generator) instead."""
+        top-k (generation/sampling.py:24-33), top-p (:34-47), softmax, multinomial draw, beam log-probability — and the
+        hand-over of the sampled token to the next step, all through device-side state.  With the fused kernel the
+        tail is ONE launch (cv_sample_topk, or cv_sample_topk_topp when top_p > 0; own counter-based generator);
+        COGVIEW_B200_FUSED_SAMPLING=0 keeps the reference's torch operations (torch.multinomial's generator) instead."""
         temperature, top_k, inv = key[:3]
+        top_p = key[5]
         logits = self._run()
         if self.sparse is not None:
             self.len64.add_(1)
@@ -217,7 +219,7 @@ class DecodeRunner:
         if os.environ.get('COGVIEW_B200_FUSED_SAMPLING', '1') != '0' and 1 <= len(valid) <= 4:
             ops.sample_topk(logits, temperature, top_k, valid, seed_dev=self.seed_dev, step=self.stepc,
                             next_ids=self.ids, out_tokens=self.out_buf, score_acc=self.score_acc, pos=self.pos,
-                            cur_len=self.cur_len, done=self.done)
+                            cur_len=self.cur_len, done=self.done, top_p=top_p)
             return
         logits = logits.clone()
         logits.div_(temperature)
@@ -226,6 +228,8 @@ class DecodeRunner:
         if top_k > 0:
             kth = torch.topk(logits, top_k)[0][..., -1, None]
             logits.masked_fill_(logits < kth, -float('Inf'))
+        if top_p > 0.0:
+            top_p_logits(logits, top_p)
         probs = F.softmax(logits, dim=-1)
         prev = torch.multinomial(probs, num_samples=1)
         self.score_acc.add_(torch.log(torch.gather(probs, 1, prev)[:, 0]))
@@ -248,9 +252,11 @@ class DecodeRunner:
             self.len64.fill_(t)
             self.plan_err.zero_()
 
-    def sample_run(self, ids, pos, t, n_steps, temperature, top_k, invalid_slices, sparse=None, row_pad=None):
+    def sample_run(self, ids, pos, t, n_steps, temperature, top_k, invalid_slices, sparse=None, row_pad=None,
+                   top_p=0.0):
         """n_steps tokens starting from `ids` ([b, 1], at positions `pos`, t tokens cached).  One graph replay per
         token.  Returns (tokens [b, n_steps] int64, summed log-probabilities [b] fp32).
+        top_p > 0: nucleus filtering after top-k.
         sparse: None, or dict(n_img=..., tokens=[b, t + 1] every token so far) for is_sparse == 2.
         row_pad: None, or int32 [b] on the device: row i holds t - row_pad[i] cached tokens (ragged mode; not with
         sparse).  In shared mode t is the suffix length and t + n_steps must fit the suffix cache."""
@@ -260,7 +266,7 @@ class DecodeRunner:
         self.last_t = t + n_steps
         vocab = self.model.word_embeddings.weight.shape[0]
         key = (float(temperature), int(top_k), tuple(sl.indices(vocab)[:2] for sl in invalid_slices),
-               None if sparse is None else int(sparse['n_img']), row_pad is not None)
+               None if sparse is None else int(sparse['n_img']), row_pad is not None, float(top_p))
         if self.shared:
             key += (self._mode(),)
         assert n_steps <= self.out_buf.shape[1]

@@ -628,9 +628,10 @@ def valid_ranges(invalid, vocab):
 
 
 def sample_topk(logits, temperature, top_k, valid, *, seed=0, seed_dev=None, step=None, next_ids=None, out_tokens=None,
-                score_acc=None, pos=None, cur_len=None, done=None, want_probs=False):
+                score_acc=None, pos=None, cur_len=None, done=None, want_probs=False, top_p=0.0):
     """Sampling tail of generation/sampling.py:157-183 in one kernel.  logits fp32 [b, V] (unchanged);
-    valid: list of [lo, hi) vocabulary ranges (<= 4).  Returns (next_ids int64 [b], probs or None)."""
+    valid: list of [lo, hi) vocabulary ranges (<= 4).  top_p > 0 adds the nucleus filter after top-k
+    (cv_sample_topk_topp); top_p == 0 runs cv_sample_topk.  Returns (next_ids int64 [b], probs or None)."""
     import ctypes
     require_cuda(logits, seed_dev, step, next_ids, out_tokens, score_acc, pos, cur_len, done)
     b, V = logits.shape
@@ -643,11 +644,14 @@ def sample_topk(logits, temperature, top_k, valid, *, seed=0, seed_dev=None, ste
         done = torch.zeros(1, dtype=torch.int32, device=logits.device)
     probs = torch.empty((b, logits.stride(0)), dtype=torch.float32, device=logits.device) if want_probs else None
     flat = (ctypes.c_int * (2 * len(valid)))(*[int(x) for r in valid for x in r])
-    rc = lib().cv_sample_topk(ptr(logits), logits.stride(0), b, V, float(temperature), int(top_k), flat, len(valid),
-                              int(seed) & 0xFFFFFFFFFFFFFFFF, ptr(seed_dev), ptr(step), ptr(next_ids), ptr(out_tokens),
-                              0 if out_tokens is None else out_tokens.stride(0), ptr(score_acc), ptr(pos), ptr(cur_len),
-                              ptr(done), ptr(probs), stream_ptr())
-    check(rc, "cv_sample_topk")
+    args = (ptr(logits), logits.stride(0), b, V, float(temperature), int(top_k), flat, len(valid),
+            int(seed) & 0xFFFFFFFFFFFFFFFF, ptr(seed_dev), ptr(step), ptr(next_ids), ptr(out_tokens),
+            0 if out_tokens is None else out_tokens.stride(0), ptr(score_acc), ptr(pos), ptr(cur_len), ptr(done),
+            ptr(probs))
+    if top_p > 0.0:
+        check(lib().cv_sample_topk_topp(*args, float(top_p), stream_ptr()), "cv_sample_topk_topp")
+    else:
+        check(lib().cv_sample_topk(*args, stream_ptr()), "cv_sample_topk")
     return next_ids, (probs[:, :V] if want_probs else None)
 
 

@@ -312,6 +312,17 @@ int cv_sample_topk(const float* logits, int64_t ld, int b, int vocab, float temp
                    int64_t* next_ids,
                    int64_t* out_tokens, int64_t ld_out, float* score_acc, int64_t* pos, int* cur_len,
                    unsigned int* done_counter, float* probs_out, void* stream);
+/* cv_sample_topk_topp: cv_sample_topk with nucleus (top-p) filtering after the top-k filter (top_k_logits :34-47):
+ *   of the top-k survivors, keep a token iff the probability mass of the tokens strictly above it (softmax over the
+ *   survivors) is <= top_p; the first token that takes the mass past top_p is kept.  Every token whose logit equals
+ *   the boundary logit is kept (torch.sort leaves the order among ties unspecified).  The mass is accumulated in
+ *   2^-40 fixed point (exact integer sums: repeated calls are bit-equal).  top_p > 0; top_p >= 1 keeps every top-k
+ *   survivor.  Draw, score and outputs as cv_sample_topk; probs_out is the renormalised distribution over the kept set. */
+int cv_sample_topk_topp(const float* logits, int64_t ld, int b, int vocab, float temperature, int top_k,
+                        const int* valid, int n_valid, uint64_t seed, const uint64_t* seed_dev, int64_t* step,
+                        int64_t* next_ids,
+                        int64_t* out_tokens, int64_t ld_out, float* score_acc, int64_t* pos, int* cur_len,
+                        unsigned int* done_counter, float* probs_out, float top_p, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Optimizer step: fused AdamW on bf16 parameters with fp32 master weights / moments — replaces
