@@ -453,12 +453,12 @@ extern "C" int64_t cv_attn_sparse_bwd_workspace_bytes(int b, int heads, int head
                      al256b((size_t)b * n_piv * 3 * h * 2) + al256b((size_t)b * n_piv * 4));
 }
 
-namespace {
-int attn_sparse_bwd(const void* q, int64_t ldq, int64_t bsq, const void* k, int64_t ldk, int64_t bsk, const void* v,
-                    int64_t ldv, int64_t bsv, const int64_t* pivot_idx, const void* out, const void* d_out,
-                    const float* lse, void* dqkv, void* workspace, int b, int heads, int head_dim, int s, int n_piv,
-                    int query_window, int key_window_times, float dropout_p, const uint32_t* drop_mask,
-                    cudaStream_t st) {
+extern "C" int cv_attn_sparse_bwd(const void* q, int64_t ldq, int64_t bsq, const void* k, int64_t ldk, int64_t bsk,
+                                  const void* v, int64_t ldv, int64_t bsv, const int64_t* pivot_idx, const void* out,
+                                  const void* d_out, const float* lse, void* dqkv, void* workspace, int b, int heads,
+                                  int head_dim, int s, int n_piv, int query_window, int key_window_times,
+                                  float dropout_p, const uint32_t* drop_mask, void* stream) {
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
     CV_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, "dropout probability must be in [0, 1)");
     CV_REQUIRE(dropout_p == 0.f || drop_mask != nullptr, "attention dropout needs the keep mask saved by the forward");
     CV_REQUIRE(q && k && v && pivot_idx && out && d_out && lse && dqkv && workspace, "null pointer");
@@ -543,26 +543,4 @@ int attn_sparse_bwd(const void* q, int64_t ldq, int64_t bsq, const void* k, int6
         CV_LAUNCH_CHECK();
     }
     return 0;
-}
-}  // namespace
-
-extern "C" int cv_attn_sparse_bwd(const void* q, int64_t ldq, int64_t bsq, const void* k, int64_t ldk, int64_t bsk,
-                                  const void* v, int64_t ldv, int64_t bsv, const int64_t* pivot_idx, const void* out,
-                                  const void* d_out, const float* lse, void* dqkv, void* workspace, int b, int heads,
-                                  int head_dim, int s, int n_piv, int query_window, int key_window_times,
-                                  void* stream) {
-    return attn_sparse_bwd(q, ldq, bsq, k, ldk, bsk, v, ldv, bsv, pivot_idx, out, d_out, lse, dqkv, workspace, b, heads,
-                           head_dim, s, n_piv, query_window, key_window_times, 0.f, nullptr,
-                           static_cast<cudaStream_t>(stream));
-}
-
-extern "C" int cv_attn_sparse_bwd_dropout(const void* q, int64_t ldq, int64_t bsq, const void* k, int64_t ldk,
-                                          int64_t bsk, const void* v, int64_t ldv, int64_t bsv, const int64_t* pivot_idx,
-                                          const void* out, const void* d_out, const float* lse, void* dqkv,
-                                          void* workspace, int b, int heads, int head_dim, int s, int n_piv,
-                                          int query_window, int key_window_times, float dropout_p,
-                                          const uint32_t* drop_mask, void* stream) {
-    return attn_sparse_bwd(q, ldq, bsq, k, ldk, bsk, v, ldv, bsv, pivot_idx, out, d_out, lse, dqkv, workspace, b, heads,
-                           head_dim, s, n_piv, query_window, key_window_times, dropout_p, drop_mask,
-                           static_cast<cudaStream_t>(stream));
 }

@@ -495,12 +495,12 @@ extern "C" int64_t cv_attn_sparse_drop_mask_words(int b, int heads, int s, int n
     return L.fwd_words + L.band_words + L.piv_words;
 }
 
-namespace {
-int attn_sparse_fwd(const void* q, int64_t ldq, int64_t bsq, const void* k, int64_t ldk, int64_t bsk, const void* v,
-                    int64_t ldv, int64_t bsv, const int64_t* pivot_idx, void* out, int64_t ldo, int64_t bso, float* lse,
-                    void* workspace, int b, int heads, int head_dim, int s, int n_piv, int query_window,
-                    int key_window_times, float dropout_p, uint64_t seed, uint32_t site, uint32_t* drop_mask,
-                    cudaStream_t st) {
+extern "C" int cv_attn_sparse_fwd(const void* q, int64_t ldq, int64_t bsq, const void* k, int64_t ldk, int64_t bsk,
+                                  const void* v, int64_t ldv, int64_t bsv, const int64_t* pivot_idx, void* out,
+                                  int64_t ldo, int64_t bso, float* lse, void* workspace, int b, int heads,
+                                  int head_dim, int s, int n_piv, int query_window, int key_window_times,
+                                  float dropout_p, uint64_t seed, uint32_t site, uint32_t* drop_mask, void* stream) {
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
     CV_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, "dropout probability must be in [0, 1)");
     CV_REQUIRE(dropout_p == 0.f || drop_mask != nullptr, "attention dropout needs the keep-mask buffer");
     CV_REQUIRE(q && k && v && pivot_idx && out && workspace, "null pointer");
@@ -559,26 +559,4 @@ int attn_sparse_fwd(const void* q, int64_t ldq, int64_t bsq, const void* k, int6
     }
     CV_LAUNCH_CHECK();
     return 0;
-}
-}  // namespace
-
-extern "C" int cv_attn_sparse_fwd(const void* q, int64_t ldq, int64_t bsq, const void* k, int64_t ldk, int64_t bsk,
-                                  const void* v, int64_t ldv, int64_t bsv, const int64_t* pivot_idx, void* out,
-                                  int64_t ldo, int64_t bso, float* lse, void* workspace, int b, int heads,
-                                  int head_dim, int s, int n_piv, int query_window, int key_window_times,
-                                  void* stream) {
-    return attn_sparse_fwd(q, ldq, bsq, k, ldk, bsk, v, ldv, bsv, pivot_idx, out, ldo, bso, lse, workspace, b, heads,
-                           head_dim, s, n_piv, query_window, key_window_times, 0.f, 0, 0, nullptr,
-                           static_cast<cudaStream_t>(stream));
-}
-
-extern "C" int cv_attn_sparse_fwd_dropout(const void* q, int64_t ldq, int64_t bsq, const void* k, int64_t ldk,
-                                          int64_t bsk, const void* v, int64_t ldv, int64_t bsv, const int64_t* pivot_idx,
-                                          void* out, int64_t ldo, int64_t bso, float* lse, void* workspace, int b,
-                                          int heads, int head_dim, int s, int n_piv, int query_window,
-                                          int key_window_times, float dropout_p, uint64_t seed, uint32_t site,
-                                          uint32_t* drop_mask, void* stream) {
-    return attn_sparse_fwd(q, ldq, bsq, k, ldk, bsk, v, ldv, bsv, pivot_idx, out, ldo, bso, lse, workspace, b, heads,
-                           head_dim, s, n_piv, query_window, key_window_times, dropout_p, seed, site, drop_mask,
-                           static_cast<cudaStream_t>(stream));
 }

@@ -1,8 +1,8 @@
 // Ragged multi-token attention on the K|V cache (cv_attn_chunk_ragged): a chunk of n new tokens per sequence attends
 // to that sequence's own cached prefix and to itself (causal inside the chunk), and the chunk's K|V is appended.
-// It is the multi-query form of cv_attn_decode_ragged (csrc/decode.cu): super-resolution templates interleave given
-// stretches of codes with generated ones, and the given stretch plus the last sampled token (17 tokens) go through
-// the model as one chunk for every image of a decode batch, each image at its own cache length.
+// It is the multi-query form of cv_attn_decode with row_pad (csrc/decode.cu): super-resolution templates interleave
+// given stretches of codes with generated ones, and the given stretch plus the last sampled token (17 tokens) go
+// through the model as one chunk for every image of a decode batch, each image at its own cache length.
 //
 // At the shapes it serves the kernel is bound by reading the cache (64 rows x ~1300 tokens x 5120 bf16 columns is
 // ~0.85 GB per layer), so the design point is that every cached key and value is read from HBM ONCE per (row, head)

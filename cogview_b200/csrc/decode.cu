@@ -7,9 +7,8 @@
 //                        generation/sampling.py:147-151, and the last-token logits GEMM, model/gpt2_modeling.py:117)
 //   cv_attn_decode    : one query per sequence against the K|V cache, with the new token's K/V appended
 //                       in the same kernel (standard_attention, mpu/sparse_transformer.py:652-673, for sq = 1,
-//                       where every cached key is visible)
-//   cv_attn_decode_ragged : the same with a cache length per sequence (t_b = cur_len - row_pad[b]), so sequences of
-//                       captions of different lengths share one decode batch
+//                       where every cached key is visible); with row_pad, a cache length per sequence
+//                       (t_b = cur_len - row_pad[b]), so captions of different lengths share one decode batch
 #include "common.cuh"
 #include "host.h"
 #include "../../include/cogview_b200.h"
@@ -630,10 +629,11 @@ extern "C" int64_t cv_attn_decode_workspace_bytes(int b, int heads, int nsplit) 
 }
 
 namespace {
-// cv_attn_decode and cv_attn_decode_ragged (row_pad == nullptr: every row holds the same cur_len tokens)
+// cv_attn_decode and cv_attn_decode_gather: attn_decode_kernel over the keys 0..t (idx == nullptr; RAGGED when
+// row_pad is non-null) or over the gathered list idx (GATHER), then, for nsplit > 1, the split-K combine kernel.
 int attn_decode_launch(const void* qkv, void* cache, int64_t cache_batch_stride, const int* cur_len_dev, int cur_len,
-                       const int* row_pad, void* out, float* workspace, int b, int heads, int head_dim, int max_len,
-                       int nsplit, void* stream) {
+                       const int* row_pad, const int* idx, int64_t idx_batch_stride, const int* n_dev, void* out,
+                       float* workspace, int b, int heads, int head_dim, int max_len, int nsplit, void* stream) {
     CV_REQUIRE(qkv && cache && out, "null pointer");
     CV_REQUIRE(head_dim == HD, "head_dim must be 64");
     CV_REQUIRE(b > 0 && heads > 0 && max_len > 0 && nsplit >= 1 && nsplit <= 64, "bad sizes");
@@ -650,10 +650,12 @@ int attn_decode_launch(const void* qkv, void* cache, int64_t cache_batch_stride,
     p.partial = workspace;
     p.heads = heads; p.nsplit = nsplit; p.max_len = max_len;
     p.scale_log2 = (1.0f / sqrtf((float)head_dim)) * 1.4426950408889634f;
-    p.idx = nullptr; p.idx_bs = 0; p.n_dev = nullptr;
+    p.idx = idx; p.idx_bs = idx_batch_stride; p.n_dev = n_dev;
     p.row_pad = row_pad;
     dim3 grid(heads, b, nsplit);
-    if (row_pad != nullptr) {
+    if (idx != nullptr) {
+        CV_CUDA(cvh::launch_pdl(attn_decode_kernel<true, false>, grid, dim3(DA_WARPS * 32), 0, s, true, p));
+    } else if (row_pad != nullptr) {
         CV_CUDA(cvh::launch_pdl(attn_decode_kernel<false, true>, grid, dim3(DA_WARPS * 32), 0, s, true, p));
     } else {
         CV_CUDA(cvh::launch_pdl(attn_decode_kernel<false, false>, grid, dim3(DA_WARPS * 32), 0, s, true, p));
@@ -669,18 +671,10 @@ int attn_decode_launch(const void* qkv, void* cache, int64_t cache_batch_stride,
 }  // namespace
 
 extern "C" int cv_attn_decode(const void* qkv, void* cache, int64_t cache_batch_stride, const int* cur_len_dev,
-                              int cur_len, void* out, float* workspace, int b, int heads, int head_dim, int max_len,
-                              int nsplit, void* stream) {
-    return attn_decode_launch(qkv, cache, cache_batch_stride, cur_len_dev, cur_len, nullptr, out, workspace, b, heads,
-                              head_dim, max_len, nsplit, stream);
-}
-
-extern "C" int cv_attn_decode_ragged(const void* qkv, void* cache, int64_t cache_batch_stride, const int* cur_len_dev,
-                                     int cur_len, const int* row_pad, void* out, float* workspace, int b, int heads,
-                                     int head_dim, int max_len, int nsplit, void* stream) {
-    CV_REQUIRE(row_pad != nullptr, "null pointer");
-    return attn_decode_launch(qkv, cache, cache_batch_stride, cur_len_dev, cur_len, row_pad, out, workspace, b, heads,
-                              head_dim, max_len, nsplit, stream);
+                              int cur_len, const int* row_pad, void* out, float* workspace, int b, int heads,
+                              int head_dim, int max_len, int nsplit, void* stream) {
+    return attn_decode_launch(qkv, cache, cache_batch_stride, cur_len_dev, cur_len, row_pad, nullptr, 0, nullptr, out,
+                              workspace, b, heads, head_dim, max_len, nsplit, stream);
 }
 
 extern "C" int cv_attn_gather(const void* q, int64_t ldq, int64_t bsq, const void* cache, int64_t cache_batch_stride,
@@ -797,30 +791,7 @@ extern "C" int cv_attn_decode_gather(const void* qkv, void* cache, int64_t cache
                                      const int* idx, int64_t idx_batch_stride, const int* n_dev, void* out,
                                      float* workspace, int b, int heads, int head_dim, int max_len, int nsplit,
                                      void* stream) {
-    CV_REQUIRE(qkv && cache && out && cur_len_dev && idx && n_dev, "null pointer");
-    CV_REQUIRE(head_dim == HD, "head_dim must be 64");
-    CV_REQUIRE(b > 0 && heads > 0 && max_len > 0 && nsplit >= 1 && nsplit <= 64, "bad sizes");
-    CV_REQUIRE(nsplit == 1 || workspace != nullptr, "workspace required when nsplit > 1");
-    cudaStream_t s = static_cast<cudaStream_t>(stream);
-    DecodeParams p;
-    p.qkv = static_cast<const __nv_bfloat16*>(qkv);
-    p.cache = static_cast<__nv_bfloat16*>(cache);
-    p.cache_bs = cache_batch_stride;
-    p.cur_len_dev = cur_len_dev;
-    p.cur_len = -1;
-    p.out = static_cast<__nv_bfloat16*>(out);
-    p.partial = workspace;
-    p.heads = heads; p.nsplit = nsplit; p.max_len = max_len;
-    p.scale_log2 = (1.0f / sqrtf((float)head_dim)) * 1.4426950408889634f;
-    p.idx = idx; p.idx_bs = idx_batch_stride; p.n_dev = n_dev;
-    p.row_pad = nullptr;
-    dim3 grid(heads, b, nsplit);
-    CV_CUDA(cvh::launch_pdl(attn_decode_kernel<true, false>, grid, dim3(DA_WARPS * 32), 0, s, true, p));
-    cvh::count_launches(1);
-    if (nsplit > 1) {
-        CV_CUDA(cvh::launch_pdl(attn_decode_combine_kernel, dim3(heads, b), dim3(HD), 0, s, true,
-                                static_cast<const float*>(workspace), static_cast<__nv_bfloat16*>(out), heads, nsplit));
-        cvh::count_launches(1);
-    }
-    return 0;
+    CV_REQUIRE(cur_len_dev && idx && n_dev, "null pointer");
+    return attn_decode_launch(qkv, cache, cache_batch_stride, cur_len_dev, -1, nullptr, idx, idx_batch_stride, n_dev,
+                              out, workspace, b, heads, head_dim, max_len, nsplit, stream);
 }

@@ -207,9 +207,10 @@ static bool split_tail_enabled() {   // COGVIEW_B200_GEMM_SPLIT_TAIL=0 disables 
     return on;
 }
 
-static int gemm_impl(const void* A, int a_mn_major, int64_t lda, const void* B, int b_mn_major, int64_t ldb,
-                     void* Cout, int c_is_f32, int64_t ldc, void* C2, const void* bias, int act, float* absmax,
-                     int M, int N, int K, int block_n, const cvh::HostDropout& hd, void* stream) {
+extern "C" int cv_gemm_bf16(const void* A, int a_mn_major, int64_t lda, const void* B, int b_mn_major, int64_t ldb,
+                            void* Cout, int c_is_f32, int64_t ldc, void* C2, const void* bias, int act, float* absmax,
+                            int M, int N, int K, int block_n, float dropout_p, uint64_t seed, uint32_t site,
+                            void* stream) {
     CV_REQUIRE(A && B && Cout, "null operand");
     CV_REQUIRE(M > 0 && N > 0 && K > 0, "M, N, K must be positive");
     CV_REQUIRE(lda % 8 == 0 && ldb % 8 == 0, "lda/ldb must be multiples of 8 elements (16-byte TMA strides)");
@@ -253,6 +254,7 @@ static int gemm_impl(const void* A, int a_mn_major, int64_t lda, const void* B, 
     p.bias = static_cast<const __nv_bfloat16*>(bias);
     p.act = act;
     p.absmax = absmax;
+    const cvh::HostDropout hd = cvh::make_dropout(dropout_p, seed, site);
     CV_REQUIRE(hd.p >= 0.f && hd.p < 1.f, "dropout probability must be in [0, 1)");
     CV_REQUIRE(hd.p == 0.f || N % 4 == 0, "dropout needs N % 4 == 0");
     p.drop.p = hd.p; p.drop.scale = hd.scale; p.drop.threshold = hd.threshold; p.drop.stream = hd.stream;
@@ -274,19 +276,4 @@ static int gemm_impl(const void* A, int a_mn_major, int64_t lda, const void* B, 
     if (rc) return rc;
     if (BN == 256) return dispatch<256>(a_mn_major, b_mn_major, c_is_f32, tmA, tmB, p, s);
     return dispatch<128>(a_mn_major, b_mn_major, c_is_f32, tmA, tmB, p, s);
-}
-
-extern "C" int cv_gemm_bf16(const void* A, int a_mn_major, int64_t lda, const void* B, int b_mn_major, int64_t ldb,
-                            void* Cout, int c_is_f32, int64_t ldc, void* C2, const void* bias, int act, float* absmax,
-                            int M, int N, int K, int block_n, void* stream) {
-    return gemm_impl(A, a_mn_major, lda, B, b_mn_major, ldb, Cout, c_is_f32, ldc, C2, bias, act, absmax, M, N, K,
-                     block_n, cvh::make_dropout(0.f, 0, 0), stream);
-}
-
-extern "C" int cv_gemm_bf16_dropout(const void* A, int a_mn_major, int64_t lda, const void* B, int b_mn_major,
-                                    int64_t ldb, void* Cout, int c_is_f32, int64_t ldc, void* C2, const void* bias,
-                                    int act, float* absmax, int M, int N, int K, int block_n, float dropout_p,
-                                    uint64_t seed, uint32_t site, void* stream) {
-    return gemm_impl(A, a_mn_major, lda, B, b_mn_major, ldb, Cout, c_is_f32, ldc, C2, bias, act, absmax, M, N, K,
-                     block_n, cvh::make_dropout(dropout_p, seed, site), stream);
 }

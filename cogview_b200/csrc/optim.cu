@@ -1,4 +1,4 @@
-// cv_adamw_step: fused AdamW on bf16 parameters with fp32 master weights and moments.
+// cv_adamw_step_multi: fused AdamW on bf16 parameters with fp32 master weights and moments.
 //
 // Replaces the optimizer sweep of the reference's training step: FP16_Optimizer.step (fp16/fp16.py:399-453:
 // copy fp16 grads to fp32 masters' .grad, unscale, step, copy masters back to fp16) around apex FusedAdam
@@ -6,87 +6,13 @@
 //   g = grad * grad_scale (grad_scale carries the clip coefficient; bf16 needs no loss scale)
 //   m = b1 m + (1-b1) g;  v = b2 v + (1-b2) g^2
 //   w = w - lr * ( (m / (1-b1^t)) / (sqrt(v / (1-b2^t)) + eps) + wd * w );   param_bf16 = round(w)
-// HBM-bound: 2+2+12 bytes read, 2+12 written per parameter; 16-byte vectorised, grid = multiple of the SM count.
+// HBM-bound: 2+2+12 bytes read, 2+12 written per parameter; 16-byte vectorised.
 #include "common.cuh"
 #include "host.h"
 #include "../../include/cogview_b200.h"
 
 namespace {
 using namespace cv;
-
-__global__ void __launch_bounds__(256)
-adamw_kernel(__nv_bfloat16* __restrict__ param, const __nv_bfloat16* __restrict__ grad, float* __restrict__ master,
-             float* __restrict__ m, float* __restrict__ v, size_t n, float lr, float beta1, float beta2, float eps,
-             float weight_decay, float bc1, float bc2, const float* __restrict__ grad_scale_dev, float grad_scale) {
-    const float gs = grad_scale_dev ? *grad_scale_dev * grad_scale : grad_scale;
-    const size_t n4 = n / 4;
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
-        uint2 gu = reinterpret_cast<const uint2*>(grad)[i];
-        const __nv_bfloat162* gp = reinterpret_cast<const __nv_bfloat162*>(&gu);
-        float g[4] = {__low2float(gp[0]) * gs, __high2float(gp[0]) * gs, __low2float(gp[1]) * gs,
-                      __high2float(gp[1]) * gs};
-        float4 w4 = reinterpret_cast<float4*>(master)[i];
-        float4 m4 = reinterpret_cast<float4*>(m)[i];
-        float4 v4 = reinterpret_cast<float4*>(v)[i];
-        float w[4] = {w4.x, w4.y, w4.z, w4.w}, mm[4] = {m4.x, m4.y, m4.z, m4.w}, vv[4] = {v4.x, v4.y, v4.z, v4.w};
-#pragma unroll
-        for (int t = 0; t < 4; ++t) {
-            mm[t] = beta1 * mm[t] + (1.f - beta1) * g[t];
-            vv[t] = beta2 * vv[t] + (1.f - beta2) * g[t] * g[t];
-            const float upd = (mm[t] / bc1) / (sqrtf(vv[t] / bc2) + eps) + weight_decay * w[t];
-            w[t] -= lr * upd;
-        }
-        reinterpret_cast<float4*>(master)[i] = make_float4(w[0], w[1], w[2], w[3]);
-        reinterpret_cast<float4*>(m)[i] = make_float4(mm[0], mm[1], mm[2], mm[3]);
-        reinterpret_cast<float4*>(v)[i] = make_float4(vv[0], vv[1], vv[2], vv[3]);
-        uint2 pu;
-        pu.x = pack_bf16x2(w[0], w[1]);
-        pu.y = pack_bf16x2(w[2], w[3]);
-        reinterpret_cast<uint2*>(param)[i] = pu;
-    }
-    // tail (n not a multiple of 4)
-    if (blockIdx.x == 0 && threadIdx.x < (n & 3)) {
-        const size_t i = n4 * 4 + threadIdx.x;
-        const float g = __bfloat162float(grad[i]) * gs;
-        float mm = beta1 * m[i] + (1.f - beta1) * g;
-        float vv = beta2 * v[i] + (1.f - beta2) * g * g;
-        float w = master[i];
-        w -= lr * ((mm / bc1) / (sqrtf(vv / bc2) + eps) + weight_decay * w);
-        m[i] = mm; v[i] = vv; master[i] = w;
-        param[i] = __float2bfloat16_rn(w);
-    }
-}
-
-// sum of squares of a bf16 tensor, accumulated (atomicAdd) into *out — for the global gradient norm
-__global__ void __launch_bounds__(256)
-sumsq_kernel(const __nv_bfloat16* __restrict__ x, size_t n, float* __restrict__ out) {
-    float s = 0.f;
-    const size_t n8 = n / 8;
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n8; i += (size_t)gridDim.x * blockDim.x) {
-        uint4 u = reinterpret_cast<const uint4*>(x)[i];
-        const __nv_bfloat162* p = reinterpret_cast<const __nv_bfloat162*>(&u);
-#pragma unroll
-        for (int t = 0; t < 4; ++t) {
-            const float a = __low2float(p[t]), b = __high2float(p[t]);
-            s += a * a + b * b;
-        }
-    }
-    if (blockIdx.x == 0 && threadIdx.x < (n & 7)) {
-        const float a = __bfloat162float(x[n8 * 8 + threadIdx.x]);
-        s += a * a;
-    }
-    s = warp_sum(s);
-    __shared__ float sh[8];
-    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = s;
-    __syncthreads();
-    if (threadIdx.x < 8) {
-        float t = sh[threadIdx.x];
-        t += __shfl_xor_sync(0xffu, t, 4);
-        t += __shfl_xor_sync(0xffu, t, 2);
-        t += __shfl_xor_sync(0xffu, t, 1);
-        if (threadIdx.x == 0) atomicAdd(out, t);
-    }
-}
 
 // clip coefficient from the accumulated sum of squares: coef = min(1, max_norm / (sqrt(sumsq) + 1e-6)).
 // A non-finite norm (one inf / NaN gradient anywhere) marks the step as skipped — the overflow branch of the
@@ -196,38 +122,7 @@ sumsq_multi_kernel(const cv_adamw_entry* __restrict__ table, float* __restrict__
     }
 }
 
-int grid_for(size_t items) {
-    size_t blocks = (items + 255) / 256;
-    size_t cap = (size_t)cvh::num_sms() * 8;
-    return (int)(blocks < cap ? (blocks ? blocks : 1) : cap);
-}
 }  // namespace
-
-extern "C" int cv_adamw_step(void* param, const void* grad, float* master, float* m, float* v, int64_t n, float lr,
-                             float beta1, float beta2, float eps, float weight_decay, int step,
-                             const float* grad_scale_dev, float grad_scale, void* stream) {
-    CV_REQUIRE(param && grad && master && m && v, "null pointer");
-    CV_REQUIRE(n > 0 && step >= 1, "n and step must be positive");
-    CV_REQUIRE((reinterpret_cast<uintptr_t>(param) & 7) == 0 && (reinterpret_cast<uintptr_t>(grad) & 7) == 0 &&
-                   (reinterpret_cast<uintptr_t>(master) & 15) == 0 && (reinterpret_cast<uintptr_t>(m) & 15) == 0 &&
-                   (reinterpret_cast<uintptr_t>(v) & 15) == 0,
-               "buffers must be 8-byte (bf16) / 16-byte (fp32) aligned");
-    const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
-    adamw_kernel<<<grid_for((size_t)n / 4 + 1), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        static_cast<__nv_bfloat16*>(param), static_cast<const __nv_bfloat16*>(grad), master, m, v, (size_t)n, lr, beta1,
-        beta2, eps, weight_decay, bc1, bc2, grad_scale_dev, grad_scale);
-    CV_LAUNCH_CHECK();
-    return 0;
-}
-
-extern "C" int cv_sumsq_bf16(const void* x, int64_t n, float* out, void* stream) {
-    CV_REQUIRE(x && out && n > 0, "bad argument");
-    CV_REQUIRE((reinterpret_cast<uintptr_t>(x) & 15) == 0, "x must be 16-byte aligned");
-    sumsq_kernel<<<grid_for((size_t)n / 8 + 1), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-        static_cast<const __nv_bfloat16*>(x), (size_t)n, out);
-    CV_LAUNCH_CHECK();
-    return 0;
-}
 
 extern "C" int cv_clip_coef(const float* sumsq, float max_norm, float* coef, float* norm_out, int* state,
                             void* stream) {

@@ -327,10 +327,12 @@ __global__ void __launch_bounds__(ST) sample_topk_kernel(const SampleParams p, c
     }
 }
 
-int launch_sample(const float* logits, int64_t ld, int b, int vocab, float temperature, int top_k, const int* valid,
-                  int n_valid, uint64_t seed, const uint64_t* seed_dev, int64_t* step, int64_t* next_ids,
-                  int64_t* out_tokens, int64_t ld_out, float* score_acc, int64_t* pos, int* cur_len,
-                  unsigned int* done_counter, float* probs_out, void* stream, bool nucleus, float top_p) {
+}  // namespace
+
+extern "C" int cv_sample_topk(const float* logits, int64_t ld, int b, int vocab, float temperature, int top_k,
+                              const int* valid, int n_valid, uint64_t seed, const uint64_t* seed_dev, int64_t* step,
+                              int64_t* next_ids, int64_t* out_tokens, int64_t ld_out, float* score_acc, int64_t* pos,
+                              int* cur_len, unsigned int* done_counter, float* probs_out, float top_p, void* stream) {
     CV_REQUIRE(logits && next_ids && valid, "null pointer");
     CV_REQUIRE(b >= 1 && vocab >= 1 && ld >= vocab, "bad sizes");
     CV_REQUIRE(n_valid >= 1 && n_valid <= 4, "1..4 valid vocabulary ranges");
@@ -353,29 +355,8 @@ int launch_sample(const float* logits, int64_t ld, int b, int vocab, float tempe
     p.nvalid = total;
     p.seed = seed; p.seed_dev = seed_dev; p.step = step; p.next_ids = next_ids; p.out_tokens = out_tokens; p.ld_out = ld_out;
     p.score_acc = score_acc; p.pos = pos; p.cur_len = cur_len; p.done = done_counter; p.probs_out = probs_out;
-    if (nucleus) sample_topk_kernel<true><<<b, ST, 0, static_cast<cudaStream_t>(stream)>>>(p, top_p);
+    if (top_p > 0.f) sample_topk_kernel<true><<<b, ST, 0, static_cast<cudaStream_t>(stream)>>>(p, top_p);
     else sample_topk_kernel<false><<<b, ST, 0, static_cast<cudaStream_t>(stream)>>>(p, 0.f);
     CV_LAUNCH_CHECK();
     return 0;
-}
-
-}  // namespace
-
-extern "C" int cv_sample_topk(const float* logits, int64_t ld, int b, int vocab, float temperature, int top_k,
-                              const int* valid, int n_valid, uint64_t seed, const uint64_t* seed_dev, int64_t* step,
-                              int64_t* next_ids,
-                              int64_t* out_tokens, int64_t ld_out, float* score_acc, int64_t* pos, int* cur_len,
-                              unsigned int* done_counter, float* probs_out, void* stream) {
-    return launch_sample(logits, ld, b, vocab, temperature, top_k, valid, n_valid, seed, seed_dev, step, next_ids,
-                         out_tokens, ld_out, score_acc, pos, cur_len, done_counter, probs_out, stream, false, 0.f);
-}
-
-extern "C" int cv_sample_topk_topp(const float* logits, int64_t ld, int b, int vocab, float temperature, int top_k,
-                                   const int* valid, int n_valid, uint64_t seed, const uint64_t* seed_dev,
-                                   int64_t* step, int64_t* next_ids, int64_t* out_tokens, int64_t ld_out,
-                                   float* score_acc, int64_t* pos, int* cur_len, unsigned int* done_counter,
-                                   float* probs_out, float top_p, void* stream) {
-    CV_REQUIRE(top_p > 0.f, "top_p must be positive (cv_sample_topk samples without the nucleus)");
-    return launch_sample(logits, ld, b, vocab, temperature, top_k, valid, n_valid, seed, seed_dev, step, next_ids,
-                         out_tokens, ld_out, score_acc, pos, cur_len, done_counter, probs_out, stream, true, top_p);
 }

@@ -6,7 +6,7 @@ it (one new token per sequence, `mems` returned by the previous call, mems_mode 
 The step runs one kernel per operation (cv_attn_decode between cv_linear_small_m / cv_ln_pair_small_m at
 batch <= 16, cv_linear_mid_m / cv_ln_pair_mid_m at batch 17..64), CUDA-graph captured; in generation runs it is
 followed by ONE sampling kernel (cv_sample_topk) inside the same graph.  In ragged mode (rows from prompts of
-different lengths, row_pad given) the attention is cv_attn_decode_ragged: row i holds cur_len - row_pad[i] cached
+different lengths, row_pad given) the attention is cv_attn_decode with row_pad: row i holds cur_len - row_pad[i] cached
 tokens.  In shared mode (a runner built on a kv_cache._SharedCaches: the beams of several prompts, each prompt's K|V
 held once) the attention is cv_attn_decode_shared over the prompts' prefix cache and the rows' own suffix cache, and
 cur_len is the suffix length.
@@ -207,7 +207,7 @@ class DecodeRunner:
         """One token: decode step, then the reference's sampling tail — temperature, invalid vocabulary slices,
         top-k (generation/sampling.py:24-33), top-p (:34-47), softmax, multinomial draw, beam log-probability — and the
         hand-over of the sampled token to the next step, all through device-side state.  With the fused kernel the
-        tail is ONE launch (cv_sample_topk, or cv_sample_topk_topp when top_p > 0; own counter-based generator);
+        tail is ONE launch (cv_sample_topk, with the nucleus filter when top_p > 0; own counter-based generator);
         COGVIEW_B200_FUSED_SAMPLING=0 keeps the reference's torch operations (torch.multinomial's generator) instead."""
         temperature, top_k, inv = key[:3]
         top_p = key[5]

@@ -44,15 +44,9 @@ def gemm(a, b, *, a_mn_major=False, b_mn_major=False, bias=None, act=ACT_NONE, o
         pre = aux
     if bias is not None:
         assert bias.dtype == torch.bfloat16 and bias.numel() == N
-    if dropout is not None and dropout[0] > 0:
-        rc = lib().cv_gemm_bf16_dropout(ptr(a), int(a_mn_major), a.stride(0), ptr(b), int(b_mn_major), b.stride(0),
-                                        ptr(out), int(out.dtype == torch.float32), out.stride(0), ptr(pre), ptr(bias),
-                                        int(act), ptr(absmax), M, N, K, block_n, float(dropout[0]), int(dropout[1]),
-                                        int(dropout[2]), stream_ptr())
-    else:
-        rc = lib().cv_gemm_bf16(ptr(a), int(a_mn_major), a.stride(0), ptr(b), int(b_mn_major), b.stride(0),
-                                ptr(out), int(out.dtype == torch.float32), out.stride(0), ptr(pre), ptr(bias), int(act),
-                                ptr(absmax), M, N, K, block_n, stream_ptr())
+    rc = lib().cv_gemm_bf16(ptr(a), int(a_mn_major), a.stride(0), ptr(b), int(b_mn_major), b.stride(0),
+                            ptr(out), int(out.dtype == torch.float32), out.stride(0), ptr(pre), ptr(bias), int(act),
+                            ptr(absmax), M, N, K, block_n, *_drop3(dropout), stream_ptr())
     check(rc, "cv_gemm_bf16")
     return (out, pre) if want_preact else out
 
@@ -189,18 +183,19 @@ def attn_sparse_fwd(q, k, v, heads, pivot_idx, query_window, key_window_times, *
     out = torch.empty((b, s, h), dtype=torch.bfloat16, device=q.device)
     lse = torch.empty((b, heads, s), dtype=torch.float32, device=q.device) if want_lse else None
     ws = torch.empty(lib().cv_attn_sparse_workspace_bytes(b, heads, 64, n_piv), dtype=torch.uint8, device=q.device)
-    args = (ptr(q), q.stride(1), q.stride(0), ptr(k), k.stride(1), k.stride(0), ptr(v), v.stride(1), v.stride(0),
-            ptr(pivot_idx), ptr(out), out.stride(1), out.stride(0), ptr(lse), ptr(ws), b, heads, 64, s, n_piv,
-            int(query_window), int(key_window_times))
     dp, dseed, dsite = _drop3(dropout)
+    mask = None
     if dp > 0:
         words = lib().cv_attn_sparse_drop_mask_words(b, heads, s, n_piv, int(query_window), int(key_window_times))
         check(words if words < 0 else 0, "cv_attn_sparse_drop_mask_words")
         mask = torch.empty(words, dtype=torch.int32, device=q.device)
-        check(lib().cv_attn_sparse_fwd_dropout(*args, dp, dseed, dsite, ptr(mask), stream_ptr()),
-              "cv_attn_sparse_fwd_dropout")
+    rc = lib().cv_attn_sparse_fwd(
+        ptr(q), q.stride(1), q.stride(0), ptr(k), k.stride(1), k.stride(0), ptr(v), v.stride(1), v.stride(0),
+        ptr(pivot_idx), ptr(out), out.stride(1), out.stride(0), ptr(lse), ptr(ws), b, heads, 64, s, n_piv,
+        int(query_window), int(key_window_times), dp, dseed, dsite, ptr(mask), stream_ptr())
+    check(rc, "cv_attn_sparse_fwd")
+    if mask is not None:
         return (out, lse, mask) if want_lse else (out, mask)
-    check(lib().cv_attn_sparse_fwd(*args, stream_ptr()), "cv_attn_sparse_fwd")
     return (out, lse) if want_lse else out
 
 
@@ -216,15 +211,14 @@ def attn_sparse_bwd(q, k, v, out, d_out, lse, heads, pivot_idx, query_window, ke
     dqkv = torch.empty((b, s, 3 * h), dtype=torch.bfloat16, device=q.device)
     ws = torch.empty(lib().cv_attn_sparse_bwd_workspace_bytes(b, heads, 64, s, n_piv), dtype=torch.uint8,
                      device=q.device)
-    args = (ptr(q), q.stride(1), q.stride(0), ptr(k), k.stride(1), k.stride(0), ptr(v), v.stride(1), v.stride(0),
-            ptr(pivot_idx), ptr(out), ptr(d_out), ptr(lse), ptr(dqkv), ptr(ws), b, heads, 64, s, n_piv,
-            int(query_window), int(key_window_times))
-    if dropout_p > 0:
+    dp = float(dropout_p) if dropout_p > 0 else 0.0
+    if dp > 0:
         require_cuda(drop_mask)
-        check(lib().cv_attn_sparse_bwd_dropout(*args, float(dropout_p), ptr(drop_mask), stream_ptr()),
-              "cv_attn_sparse_bwd_dropout")
-    else:
-        check(lib().cv_attn_sparse_bwd(*args, stream_ptr()), "cv_attn_sparse_bwd")
+    rc = lib().cv_attn_sparse_bwd(
+        ptr(q), q.stride(1), q.stride(0), ptr(k), k.stride(1), k.stride(0), ptr(v), v.stride(1), v.stride(0),
+        ptr(pivot_idx), ptr(out), ptr(d_out), ptr(lse), ptr(dqkv), ptr(ws), b, heads, 64, s, n_piv,
+        int(query_window), int(key_window_times), dp, ptr(drop_mask), stream_ptr())
+    check(rc, "cv_attn_sparse_bwd")
     return dqkv
 
 
@@ -458,7 +452,7 @@ def attn_decode(qkv, cache, heads, *, cur_len=None, cur_len_dev=None, nsplit=1, 
                 row_pad=None):
     """qkv: [b, 3h] bf16; cache: [b, max_len, 2h] bf16 (K|V); appends the new token at cur_len and returns
     the attention context [b, h] bf16.  row_pad (int32 [b] on the device, 0 <= row_pad[i] <= cur_len): row i holds
-    cur_len - row_pad[i] cached tokens and appends there (cv_attn_decode_ragged)."""
+    cur_len - row_pad[i] cached tokens and appends there."""
     require_cuda(qkv, cache, row_pad)
     b, h3 = qkv.shape
     h = h3 // 3
@@ -471,12 +465,8 @@ def attn_decode(qkv, cache, heads, *, cur_len=None, cur_len_dev=None, nsplit=1, 
     cl = -1 if cur_len is None else int(cur_len)
     if row_pad is not None:
         assert row_pad.dtype == torch.int32 and row_pad.is_contiguous() and row_pad.numel() == b
-        rc = lib().cv_attn_decode_ragged(ptr(qkv), ptr(cache), cache.stride(0), ptr(cur_len_dev), cl, ptr(row_pad),
-                                         ptr(out), ptr(workspace), b, heads, 64, cache.shape[1], nsplit, stream_ptr())
-        check(rc, "cv_attn_decode_ragged")
-        return out
-    rc = lib().cv_attn_decode(ptr(qkv), ptr(cache), cache.stride(0), ptr(cur_len_dev), cl, ptr(out), ptr(workspace), b,
-                              heads, 64, cache.shape[1], nsplit, stream_ptr())
+    rc = lib().cv_attn_decode(ptr(qkv), ptr(cache), cache.stride(0), ptr(cur_len_dev), cl, ptr(row_pad), ptr(out),
+                              ptr(workspace), b, heads, 64, cache.shape[1], nsplit, stream_ptr())
     check(rc, "cv_attn_decode")
     return out
 
@@ -630,8 +620,8 @@ def valid_ranges(invalid, vocab):
 def sample_topk(logits, temperature, top_k, valid, *, seed=0, seed_dev=None, step=None, next_ids=None, out_tokens=None,
                 score_acc=None, pos=None, cur_len=None, done=None, want_probs=False, top_p=0.0):
     """Sampling tail of generation/sampling.py:157-183 in one kernel.  logits fp32 [b, V] (unchanged);
-    valid: list of [lo, hi) vocabulary ranges (<= 4).  top_p > 0 adds the nucleus filter after top-k
-    (cv_sample_topk_topp); top_p == 0 runs cv_sample_topk.  Returns (next_ids int64 [b], probs or None)."""
+    valid: list of [lo, hi) vocabulary ranges (<= 4).  top_p > 0 adds the nucleus filter after top-k.
+    Returns (next_ids int64 [b], probs or None)."""
     import ctypes
     require_cuda(logits, seed_dev, step, next_ids, out_tokens, score_acc, pos, cur_len, done)
     b, V = logits.shape
@@ -644,14 +634,11 @@ def sample_topk(logits, temperature, top_k, valid, *, seed=0, seed_dev=None, ste
         done = torch.zeros(1, dtype=torch.int32, device=logits.device)
     probs = torch.empty((b, logits.stride(0)), dtype=torch.float32, device=logits.device) if want_probs else None
     flat = (ctypes.c_int * (2 * len(valid)))(*[int(x) for r in valid for x in r])
-    args = (ptr(logits), logits.stride(0), b, V, float(temperature), int(top_k), flat, len(valid),
-            int(seed) & 0xFFFFFFFFFFFFFFFF, ptr(seed_dev), ptr(step), ptr(next_ids), ptr(out_tokens),
-            0 if out_tokens is None else out_tokens.stride(0), ptr(score_acc), ptr(pos), ptr(cur_len), ptr(done),
-            ptr(probs))
-    if top_p > 0.0:
-        check(lib().cv_sample_topk_topp(*args, float(top_p), stream_ptr()), "cv_sample_topk_topp")
-    else:
-        check(lib().cv_sample_topk(*args, stream_ptr()), "cv_sample_topk")
+    rc = lib().cv_sample_topk(ptr(logits), logits.stride(0), b, V, float(temperature), int(top_k), flat, len(valid),
+                              int(seed) & 0xFFFFFFFFFFFFFFFF, ptr(seed_dev), ptr(step), ptr(next_ids), ptr(out_tokens),
+                              0 if out_tokens is None else out_tokens.stride(0), ptr(score_acc), ptr(pos), ptr(cur_len),
+                              ptr(done), ptr(probs), float(top_p), stream_ptr())
+    check(rc, "cv_sample_topk")
     return next_ids, (probs[:, :V] if want_probs else None)
 
 

@@ -22,7 +22,7 @@
 extern "C" {
 #endif
 
-#define CV_B200_VERSION 100
+#define CV_B200_VERSION 101
 
 int cv_version(void);
 const char* cv_last_error(void);
@@ -45,17 +45,13 @@ int cv_set_reserved_sms(int k);
  *   absmax: NULL or device float (must hold a non-negative value): atomic max of |C| — feeds the
  *           reference's abs-max pre-scaled LayerNorm (mpu/sparse_transformer.py:40-44)
  *   block_n: 0 = auto, or 128 / 256
+ *   dropout_p > 0: output dropout fused after bias/activation (output_dropout of mpu/sparse_transformer.py:167 and
+ *         :233): element (m, n) is kept iff the counter-based generator of site (seed, site) says so, kept values are
+ *         scaled by 1/(1-p); abs-max is taken after the dropout.  N % 4 == 0.  dropout_p == 0: no dropout.
  * ---------------------------------------------------------------------------------------------- */
 int cv_gemm_bf16(const void* A, int a_mn_major, int64_t lda, const void* B, int b_mn_major, int64_t ldb,
                  void* C, int c_is_f32, int64_t ldc, void* C2, const void* bias, int act, float* absmax,
-                 int M, int N, int K, int block_n, void* stream);
-/* same, with output dropout fused after bias/activation (output_dropout of mpu/sparse_transformer.py:167 and :233):
- * element (m, n) is kept iff the counter-based generator of site (seed, site) says so, kept values are scaled by
- * 1/(1-p); abs-max is taken after the dropout.  N % 4 == 0. */
-int cv_gemm_bf16_dropout(const void* A, int a_mn_major, int64_t lda, const void* B, int b_mn_major, int64_t ldb,
-                         void* C, int c_is_f32, int64_t ldc, void* C2, const void* bias, int act, float* absmax,
-                         int M, int N, int K, int block_n, float dropout_p, uint64_t seed, uint32_t site,
-                         void* stream);
+                 int M, int N, int K, int block_n, float dropout_p, uint64_t seed, uint32_t site, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Abs-max pre-scaled LayerNorm: y = LN(x / (max|x|/8)) * gamma + beta (+ residual)
@@ -160,13 +156,15 @@ int64_t cv_attn_sparse_workspace_bytes(int b, int heads, int head_dim, int n_piv
 int cv_attn_sparse_fwd(const void* q, int64_t ldq, int64_t bsq, const void* k, int64_t ldk, int64_t bsk, const void* v,
                        int64_t ldv, int64_t bsv, const int64_t* pivot_idx, void* out, int64_t ldo, int64_t bso,
                        float* lse, void* workspace, int b, int heads, int head_dim, int s, int n_piv, int query_window,
-                       int key_window_times, void* stream);
+                       int key_window_times, float dropout_p, uint64_t seed, uint32_t site, uint32_t* drop_mask,
+                       void* stream);
 int64_t cv_attn_sparse_bwd_workspace_bytes(int b, int heads, int head_dim, int s, int n_piv);
 int cv_attn_sparse_bwd(const void* q, int64_t ldq, int64_t bsq, const void* k, int64_t ldk, int64_t bsk, const void* v,
                        int64_t ldv, int64_t bsv, const int64_t* pivot_idx, const void* out, const void* d_out,
                        const float* lse, void* dqkv, void* workspace, int b, int heads, int head_dim, int s, int n_piv,
-                       int query_window, int key_window_times, void* stream);
-/* The same with dropout on the joint pivot + band probabilities (attention_dropout of mpu/sparse_transformer.py:719-721):
+                       int query_window, int key_window_times, float dropout_p, const uint32_t* drop_mask,
+                       void* stream);
+/* dropout_p > 0: dropout on the joint pivot + band probabilities (attention_dropout of mpu/sparse_transformer.py:719-721):
  * the row sum and lse stay undropped, the 1/(1-p) scale is applied once to the output row, and the backward sends dP and
  * dV through the keep bits.  The keep decision of (query i, key) is a pure function of (seed, site, batch, head, i,
  * virtual key), where the virtual keys are the s sequence positions (band keys) followed by the n_piv pivot SLOTS: pivot
@@ -184,18 +182,9 @@ int cv_attn_sparse_bwd(const void* q, int64_t ldq, int64_t bsq, const void* k, i
  *            TQ = the largest i_end(kb) - kb + 1.
  *     [piv]  key-major [b, heads, npb*128 (pivot slot), NP, 4]: bit t of word g of (pivot p, slot u) is query
  *            128 (i0 + u) + 32g + t, i0 = (times*w) / 128; NP = nqb - i0 when times*w < s, else 0 (no query sees a pivot).
- *   Entries that neither kernel reads are left unwritten. */
+ *   Entries that neither kernel reads are left unwritten.
+ * dropout_p == 0: no dropout; drop_mask may be NULL. */
 int64_t cv_attn_sparse_drop_mask_words(int b, int heads, int s, int n_piv, int query_window, int key_window_times);
-int cv_attn_sparse_fwd_dropout(const void* q, int64_t ldq, int64_t bsq, const void* k, int64_t ldk, int64_t bsk,
-                               const void* v, int64_t ldv, int64_t bsv, const int64_t* pivot_idx, void* out, int64_t ldo,
-                               int64_t bso, float* lse, void* workspace, int b, int heads, int head_dim, int s, int n_piv,
-                               int query_window, int key_window_times, float dropout_p, uint64_t seed, uint32_t site,
-                               uint32_t* drop_mask, void* stream);
-int cv_attn_sparse_bwd_dropout(const void* q, int64_t ldq, int64_t bsq, const void* k, int64_t ldk, int64_t bsk,
-                               const void* v, int64_t ldv, int64_t bsv, const int64_t* pivot_idx, const void* out,
-                               const void* d_out, const float* lse, void* dqkv, void* workspace, int b, int heads,
-                               int head_dim, int s, int n_piv, int query_window, int key_window_times, float dropout_p,
-                               const uint32_t* drop_mask, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Decode (one new token per sequence): HBM-bound weight streaming, CUDA cores.
@@ -205,7 +194,12 @@ int cv_attn_sparse_bwd_dropout(const void* q, int64_t ldq, int64_t bsq, const vo
  *   cv_attn_decode: standard_attention (mpu/sparse_transformer.py:652-673) for sq = 1 over a K|V cache
  *     [b, max_len, 2*heads*64]; qkv [b, 3*heads*64] holds q | k_new | v_new of the token at position cur_len,
  *     which is appended to the cache by the same kernel.  cur_len comes from *cur_len_dev when non-NULL
- *     (so a captured CUDA graph can be replayed), else from cur_len.  out [b, heads*64] bf16.
+ *     (so a captured CUDA graph can be replayed), else from cur_len.  out [b, heads*64] bf16.  row_pad (device int32
+ *     [b] or NULL) gives a cache length per sequence, for a batch whose rows come from prompts of different lengths:
+ *     row b holds t_b = cur_len - row_pad[b] cached tokens (cur_len: the longest row), attends over its keys 0..t_b,
+ *     the new token last, and appends its K|V at slot t_b; slots above t_b are neither read nor written.  Contract:
+ *     0 <= row_pad[b] <= cur_len and t_b < max_len.  With row_pad all zero, out and cache are bit-identical to
+ *     row_pad == NULL at the same nsplit.
  * ---------------------------------------------------------------------------------------------- */
 int cv_linear_small_m(const void* x, int64_t ldx, const void* W, int64_t ldw, const void* bias, void* out,
                       int64_t ldo, int out_is_f32, int act, float* absmax, int M, int N, int K, void* stream);
@@ -234,16 +228,8 @@ int cv_attn_gather(const void* q, int64_t ldq, int64_t bsq, const void* cache, i
                    const int64_t* idx, void* out, int b, int heads, int head_dim, int sq, int n, void* stream);
 int64_t cv_attn_decode_workspace_bytes(int b, int heads, int nsplit);
 int cv_attn_decode(const void* qkv, void* cache, int64_t cache_batch_stride, const int* cur_len_dev, int cur_len,
-                   void* out, float* workspace, int b, int heads, int head_dim, int max_len, int nsplit,
-                   void* stream);
-/* cv_attn_decode with a cache length per sequence, for a batch whose rows come from prompts of different lengths:
- * row_pad is device int32 [b], and row b holds t_b = cur_len - row_pad[b] cached tokens (cur_len from *cur_len_dev
- * when non-NULL, else cur_len: the longest row).  Row b attends over its keys 0..t_b, the new token last, and appends
- * its K|V at slot t_b; slots above t_b are neither read nor written.  Contract: 0 <= row_pad[b] <= cur_len and
- * t_b < max_len.  With row_pad all zero, out and cache are bit-identical to cv_attn_decode at the same nsplit. */
-int cv_attn_decode_ragged(const void* qkv, void* cache, int64_t cache_batch_stride, const int* cur_len_dev, int cur_len,
-                          const int* row_pad, void* out, float* workspace, int b, int heads, int head_dim, int max_len,
-                          int nsplit, void* stream);
+                   const int* row_pad, void* out, float* workspace, int b, int heads, int head_dim, int max_len,
+                   int nsplit, void* stream);
 /* Ragged multi-token attention on the K|V cache (csrc/attn_chunk.cu): a chunk of n new tokens per sequence.
  * qkv [b, n, 3h] bf16 is the packed QKV GEMM output (q | k | v per token, token-major, read in place); cache
  * [b, max_len, 2h] bf16 (K | V) with batch stride cache_batch_stride elements; row_pad device int32 [b] or NULL.
@@ -306,36 +292,26 @@ int cv_attn_decode_gather(const void* qkv, void* cache, int64_t cache_batch_stri
  *   [b, ld_out] column *step <- the draw; score_acc fp32 [b] += log p(draw); pos int64 [b] += 1; cur_len int32 += 1;
  *   step int64 += 1 (the shared scalars are advanced by the last CTA to finish); probs_out fp32 [b, ld] (testing):
  *   the full post-filter distribution.
+ *   top_p > 0: nucleus (top-p) filtering after the top-k filter (top_k_logits :34-47): of the top-k survivors, keep a
+ *   token iff the probability mass of the tokens strictly above it (softmax over the survivors) is <= top_p; the first
+ *   token that takes the mass past top_p is kept.  Every token whose logit equals the boundary logit is kept
+ *   (torch.sort leaves the order among ties unspecified).  The mass is accumulated in 2^-40 fixed point (exact integer
+ *   sums: repeated calls are bit-equal).  top_p >= 1 keeps every top-k survivor; top_p <= 0: no nucleus filter.
  * ---------------------------------------------------------------------------------------------- */
 int cv_sample_topk(const float* logits, int64_t ld, int b, int vocab, float temperature, int top_k,
                    const int* valid, int n_valid, uint64_t seed, const uint64_t* seed_dev, int64_t* step,
-                   int64_t* next_ids,
-                   int64_t* out_tokens, int64_t ld_out, float* score_acc, int64_t* pos, int* cur_len,
-                   unsigned int* done_counter, float* probs_out, void* stream);
-/* cv_sample_topk_topp: cv_sample_topk with nucleus (top-p) filtering after the top-k filter (top_k_logits :34-47):
- *   of the top-k survivors, keep a token iff the probability mass of the tokens strictly above it (softmax over the
- *   survivors) is <= top_p; the first token that takes the mass past top_p is kept.  Every token whose logit equals
- *   the boundary logit is kept (torch.sort leaves the order among ties unspecified).  The mass is accumulated in
- *   2^-40 fixed point (exact integer sums: repeated calls are bit-equal).  top_p > 0; top_p >= 1 keeps every top-k
- *   survivor.  Draw, score and outputs as cv_sample_topk; probs_out is the renormalised distribution over the kept set. */
-int cv_sample_topk_topp(const float* logits, int64_t ld, int b, int vocab, float temperature, int top_k,
-                        const int* valid, int n_valid, uint64_t seed, const uint64_t* seed_dev, int64_t* step,
-                        int64_t* next_ids,
-                        int64_t* out_tokens, int64_t ld_out, float* score_acc, int64_t* pos, int* cur_len,
-                        unsigned int* done_counter, float* probs_out, float top_p, void* stream);
+                   int64_t* next_ids, int64_t* out_tokens, int64_t ld_out, float* score_acc, int64_t* pos, int* cur_len,
+                   unsigned int* done_counter, float* probs_out, float top_p, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Optimizer step: fused AdamW on bf16 parameters with fp32 master weights / moments — replaces
  * FP16_Optimizer.step + apex FusedAdam (fp16/fp16.py:399-453, pretrain_gpt2.py:139-140; decoupled weight decay)
- * and, with cv_sumsq_bf16 + cv_clip_coef, the global-norm clipping of mpu/grads.py:28-74.
- *   grad_scale_dev: NULL or device float multiplied into the gradient (the clip coefficient); step >= 1.
+ * and, with cv_sumsq_bf16_multi + cv_clip_coef, the global-norm clipping of mpu/grads.py:28-74.
+ * One launch over a device-resident table (the whole parameter list of a model).
+ *   grad_scale_dev: NULL or device float multiplied into the gradient (the clip coefficient).
+ *   param / grad 8-byte aligned, master / m / v 16-byte aligned (for cv_sumsq_bf16_multi, grad 16-byte aligned);
+ *   bias_correction{1,2} = 1 - beta{1,2}^step, step >= 1.
  * ---------------------------------------------------------------------------------------------- */
-int cv_adamw_step(void* param, const void* grad, float* master, float* m, float* v, int64_t n, float lr, float beta1,
-                  float beta2, float eps, float weight_decay, int step, const float* grad_scale_dev,
-                  float grad_scale, void* stream);
-int cv_sumsq_bf16(const void* x, int64_t n, float* out, void* stream);   /* *out += sum(x^2) */
-/* Multi-tensor forms: one launch over a device-resident table (the whole parameter list of a model).
- * Pointers must be aligned as for cv_adamw_step / cv_sumsq_bf16; bias_correction{1,2} = 1 - beta{1,2}^step. */
 typedef struct cv_adamw_entry {
     void* param;          /* bf16 [n] */
     const void* grad;     /* bf16 [n] */
@@ -352,7 +328,8 @@ typedef struct cv_adamw_entry {
  * instead of the table. */
 int cv_adamw_step_multi(const cv_adamw_entry* table_dev, int count, float beta1, float beta2, float eps,
                         const float* grad_scale_dev, float grad_scale, const int* state, void* stream);
-int cv_sumsq_bf16_multi(const cv_adamw_entry* table_dev, int count, float* out, void* stream); /* over .grad/.n */
+/* *out += sum(grad^2) over .grad / .n of every entry */
+int cv_sumsq_bf16_multi(const cv_adamw_entry* table_dev, int count, float* out, void* stream);
 int cv_clip_coef(const float* sumsq, float max_norm, float* coef, float* norm_out, int* state, void* stream);
 
 /* ------------------------------------------------------------------------------------------------

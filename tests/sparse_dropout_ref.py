@@ -4,8 +4,9 @@
   dropout applied where the reference applies it (:719-721): probs * keep / (1 - p) after the joint softmax.  keep is a
   [b, heads, s, n_piv + w*times] 0/1 tensor in the reference's probability layout (pivot columns, then window columns);
   with keep = None it is the oracle unchanged.
-* `keep_layout` / `decode_keep`: the keep-bit buffer of cv_attn_sparse_fwd_dropout (layout in include/cogview_b200.h)
-  decoded into per-(query, virtual key) decisions, and converted to the reference layout by `to_reference_layout`.
+* `keep_layout` / `decode_keep`: the keep-bit buffer of cv_attn_sparse_fwd with dropout (layout in
+  include/cogview_b200.h) decoded into per-(query, virtual key) decisions, and converted to the reference layout by
+  `to_reference_layout`.
 """
 import math
 
@@ -51,7 +52,7 @@ def band_start(i, w, times):
 
 
 def keep_layout(b, heads, s, n_piv, w, times):
-    """The tile walk of include/cogview_b200.h (cv_attn_sparse_fwd_dropout) restated in Python."""
+    """The tile walk of include/cogview_b200.h (cv_attn_sparse_fwd with dropout) restated in Python."""
     nqb = nkb = (s + T - 1) // T
     npb = (n_piv + T - 1) // T
     last = [min(qb * T + T, s) - 1 for qb in range(nqb)]

@@ -1,4 +1,4 @@
-"""GPU tests of sampling several captions in one decode batch: cv_attn_decode_ragged (a cache length per row), the
+"""GPU tests of sampling several captions in one decode batch: cv_attn_decode with row_pad (a cache length per row), the
 DecodeRunner's ragged mode, and filling_sequences end to end.
 
 Tolerances: the kernel against a float64 softmax over each row's own keys, to one bf16 rounding of the output
@@ -27,7 +27,7 @@ def ops():
 
 
 # ----------------------------------------------------------------------------------------------------
-# 1. cv_attn_decode_ragged
+# 1. cv_attn_decode with row_pad
 # ----------------------------------------------------------------------------------------------------
 def _pads(b, cur_len, nsplit, g):
     """Row 0: no pad; row 1: the whole cache (t_b = 0); row 2: more than one split's share; the rest random."""

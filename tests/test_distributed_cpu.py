@@ -59,9 +59,11 @@ def test_dp_wrapper_and_groups_world2():
     assert sorted(out.keys()) == [0, 1]
 
 
-def test_c_abi_exports_every_declared_symbol():
-    """No GPU needed: the library loads and exports every symbol include/cogview_b200.h declares."""
+def test_c_abi_exports_exactly_the_declared_symbols():
+    """No GPU needed: the library loads, and the cv_ symbols it exports are exactly those include/cogview_b200.h
+    declares."""
     import re
+    import subprocess
     from cogview_b200 import _lib
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     header = open(os.path.join(root, "include", "cogview_b200.h")).read()
@@ -70,7 +72,11 @@ def test_c_abi_exports_every_declared_symbol():
     lib = _lib.lib()
     for n in names:
         assert hasattr(lib, n), n
-    assert lib.cv_version() == 100
+    nm = subprocess.run(["nm", "-D", "--defined-only", _lib.LIB_PATH], capture_output=True, text=True, check=True)
+    exported = sorted(s for s in (line.split()[-1] for line in nm.stdout.splitlines() if line.strip())
+                      if s.startswith("cv_"))
+    assert exported == names
+    assert lib.cv_version() == 101
 
 
 def test_product_path_refuses_cpu_tensors():

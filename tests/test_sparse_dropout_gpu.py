@@ -1,8 +1,8 @@
 """Attention-probability dropout of sparse TRAINING attention (is_sparse = 1; the reference applies attention_dropout to
-the joint pivot + window probabilities, mpu/sparse_transformer.py:150, :719-721) — cv_attn_sparse_fwd_dropout /
-cv_attn_sparse_bwd_dropout.  As for the dense sites (tests/test_dropout_gpu.py) bitwise parity with torch's generator is
-not defined; these tests pin the semantics: the kernels against the oracle run with the kernels' own keep bits, the keep
-statistics, and mask replay under activation checkpointing.
+the joint pivot + window probabilities, mpu/sparse_transformer.py:150, :719-721) — cv_attn_sparse_fwd /
+cv_attn_sparse_bwd with dropout_p > 0.  As for the dense sites (tests/test_dropout_gpu.py) bitwise parity with torch's
+generator is not defined; these tests pin the semantics: the kernels against the oracle run with the kernels' own keep
+bits, the keep statistics, and mask replay under activation checkpointing.
 Tolerances as tests/test_sparse_attention_gpu.py: 2e-2 of the output scale forward, 4e-2 of each gradient's scale."""
 import functools
 import os

@@ -84,7 +84,7 @@ def test_attn_chunk_ragged(ops, n, b, heads):
                 want = before[r].clone()
                 want[t[r]:t[r] + n, :h], want[t[r]:t[r] + n, h:] = k_new[r], v_new[r]
                 assert torch.equal(c[r].view(torch.int16), want.view(torch.int16)), (nsplit, r, t[r])
-        if n == 1:       # one query per row: cv_attn_decode_ragged's result, within tolerance
+        if n == 1:       # one query per row: cv_attn_decode's result with row_pad, within tolerance
             c = before.clone()
             dec = ops.attn_decode(qkv.view(b, 3 * h), c, heads, cur_len=cur_len, row_pad=pads.cuda())
             for nsplit, out in outs.items():

@@ -1,6 +1,6 @@
 """GPU tests of nucleus (top-p) sampling: the NUCLEUS instantiation of the fused sampling kernel
-(cv_sample_topk_topp, csrc/sample.cu) and filling_sequence with several beams and top_p > 0 on the graph-replayed
-decode path.
+(cv_sample_topk with top_p > 0, csrc/sample.cu) and filling_sequence with several beams and top_p > 0 on the
+graph-replayed decode path.
 
 * The kernel against a float64 restatement of the rule (top_k_logits, generation/sampling.py:24-49): after the
   temperature, the invalid slices and top-k, a token survives iff the softmax mass of the tokens strictly above it is

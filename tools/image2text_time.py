@@ -13,7 +13,7 @@ Seeded weights (max_memory_length 1089, as scripts/image2text.sh's --max-positio
              each image's prompt K|V is read once for all of its beams (cv_attn_decode_shared).
 Per route: total ms, s per image, and the prompt forwards and the decode runs, each call timed between device
 synchronises (so the split sums to a little less than the total): prompt-forward ms and decode ms per step.  Then
-cv_attn_decode_shared against cv_attn_decode_ragged on copied prefixes (8 groups x 8 rows, 40 heads, P = 1028,
+cv_attn_decode_shared against cv_attn_decode with row_pad on copied prefixes (8 groups x 8 rows, 40 heads, P = 1028,
 s = 10), CUDA events over 200 launches each: the K|V bytes each kernel must read and GB/s against 3350 GB/s.  The
 card's name and power limit are read in the same run.  One JSON line per measurement.  Needs a GPU.
 """
@@ -130,9 +130,9 @@ def time_kernels(cfg, where, groups=8, G=8, P=1028, s=10, reps=200):
         cv_attn_decode_shared=(lambda: ops.attn_decode_shared(qkv, prefix, suffix, heads, P, s_dev=s_dev,
                                                               nsplit=nsplit_shared),
                                (groups * P + b * (s + 1)) * 2 * h * 2, nsplit_shared),
-        cv_attn_decode_ragged=(lambda: ops.attn_decode(qkv, cache, heads, cur_len_dev=cur, nsplit=nsplit_ragged,
-                                                       row_pad=pads),
-                               b * (P + s + 1) * 2 * h * 2, nsplit_ragged))
+        cv_attn_decode=(lambda: ops.attn_decode(qkv, cache, heads, cur_len_dev=cur, nsplit=nsplit_ragged,
+                                                row_pad=pads),
+                        b * (P + s + 1) * 2 * h * 2, nsplit_ragged))
     for name, (fn, nbytes, nsplit) in runs.items():
         for _ in range(10):
             fn()

@@ -2,7 +2,7 @@
 
     python tools/top_p_time.py [--batches 1,8,16,64] [--launches 200] [--e2e 4,16,64] [--gen 512] [--reps 2]
 
-Kernel: cv_sample_topk_topp (top_p 0.9) and cv_sample_topk on the same fp32 [b, 58240] logits (randn x 3), over the
+Kernel: cv_sample_topk at top_p 0.9 and at top_p 0 on the same fp32 [b, 58240] logits (randn x 3), over the
 8192 image codes and over the text range, top_k 0 and 200; each timed with CUDA events over `--launches` launches,
 the two alternated three times, the fastest window kept.  End to end: filling_sequence on the 4B shape (seeded
 weights, bench.py's 65-token text2image context) with `--gen` generated tokens per sequence at nb beams, top_k 200,
