@@ -8,8 +8,8 @@ import torch
 
 from . import vqvae
 from .generation.magnify import magnify, magnify_batch
-from .generation.sampling import (add_interlacing_beam_marks, filling_sequence, filling_sequences,
-                                  filling_shared_prompts, get_tokenizer, inverse_prompt_score,
+from .generation.sampling import (add_interlacing_beam_marks, filling_completions, filling_sequence,
+                                  filling_sequences, filling_shared_prompts, get_tokenizer, inverse_prompt_score,
                                   inverse_prompt_scores)
 
 # generate_samples.py:203-214
@@ -183,6 +183,62 @@ def image2text(model, vq_model, args, images, num=8, fill=filling_shared_prompts
     for r in rows:
         r = torch.cat(r, dim=0)
         out.append((r, [caption_ids(row, tok) for row in r]))
+    return out
+
+
+def code_mask(pixel_mask):
+    """A [N, 256, 256] pixel mask (True: regenerate) as the [N, 32, 32] mask of the codes of a 32 x 32 grid: a code is
+    regenerated if any pixel of its 8 x 8 cell is masked."""
+    n = pixel_mask.shape[0]
+    assert tuple(pixel_mask.shape[1:]) == (256, 256), 'pixel masks are [N, 256, 256]'
+    return pixel_mask.bool().view(n, 32, 8, 32, 8).any(dim=4).any(dim=2)
+
+
+def completion_query(text, codes, mask, tokenizer=None):
+    """The template that completes one image from its caption: [ROI1] text [BASE] [BOI1] codes, with -1 (generate) at
+    every code where `mask` is True.  text: text ids (already offset into the unified vocabulary); codes: 1024 codes
+    of a 32 x 32 grid in raster order; mask: [32, 32] or [1024] bool.  A mask of the codes after the first N gives
+    build_query's '[ROI1] {} [BASE] [BOI1] [ImageN]{}' template.  Returns a list of ints."""
+    codes = [int(x) for x in codes]
+    mask = [bool(x) for x in torch.as_tensor(mask).reshape(-1).tolist()]
+    assert len(codes) == len(mask) == 1024, 'completion works on 32 x 32 code grids'
+    head = build_query('[ROI1] {} [BASE] [BOI1]', [text], tokenizer)
+    return head + [-1 if m else c for c, m in zip(codes, mask)]
+
+
+def complete_images(model, vq_model, args, texts, codes, masks, num=1, fill=filling_completions, decode=None):
+    """The reference's "text and part of image" mode for many images: image i is completed from its caption texts[i]
+    (text ids, already offset into the unified vocabulary) and the codes codes[i] ([N, 1024] int64, e.g.
+    vqvae.img2code of the images) that masks[i] ([N, 32, 32] bool, True: regenerate; see code_mask) keeps.  Each
+    image's template is completion_query's, with `num` beams marked as the reference marks them, nb = min(num,
+    args.max_inference_batch_size), and whole images are packed into batches of at most args.max_inference_batch_size
+    rows.  `fill` takes a list of templates and returns a list of token tensors: filling_completions runs the images of
+    a batch as one ragged decode whatever their masks, and falls back to filling_sequence per template where it does
+    not apply.  Every unmasked code is returned as given; the masked ones are drawn.  Returns one (token rows
+    [num, len], images [num, 3, 256, 256]) pair per image, as generate_images_batch does."""
+    decode = decode or (lambda c: vqvae.code2img(vq_model, c))
+    tok = get_tokenizer(args)
+    mbz = args.max_inference_batch_size
+    assert num < mbz or num % mbz == 0
+    assert len(texts) == codes.shape[0] == masks.shape[0], 'one text, code grid and mask per image'
+    nb = min(num, mbz)
+    per_batch = max(1, mbz // nb)
+    seqs = []
+    for text, c, m in zip(texts, codes, masks):
+        seq = torch.tensor(completion_query(text, c, m, tok), dtype=torch.long, device=codes.device)
+        add_interlacing_beam_marks(seq, nb=nb)
+        seqs.append(seq)
+    rows = [[] for _ in seqs]
+    model.eval()
+    with torch.no_grad():
+        for g0 in range(0, len(seqs), per_batch):
+            for _ in range(max(num // mbz, 1)):
+                for i, r in enumerate(fill(model, [seq.clone() for seq in seqs[g0:g0 + per_batch]], args)):
+                    rows[g0 + i].append(r)
+        out = []
+        for r in rows:
+            r = torch.cat(r, dim=0)
+            out.append((r, _decode_rows(r, decode)))
     return out
 
 

@@ -527,6 +527,100 @@ def filling_sequences(model, seqs, args):
     return out
 
 
+def _completion_plan(model, tmpls, args, tokenizer):
+    """The decode window of every template for filling_completions, and whether it can run them as one decode batch.
+    Template r's first and last generate slots are f_r and l_r; S = max_r (l_r - f_r + 1) is the number of decode
+    steps; row r's window starts at c_r = max(2, l_r + 1 - S) <= f_r.  Its tokens [0, c_r - 1) are prefilled; decode
+    step j feeds token c_r - 1 + j and yields slot c_r + j, so the S steps cover slots c_r .. c_r + S - 1, which hold
+    every generate slot of the row; the given tokens among them are forced, those after them only copied.
+    Returns (plans, S, ok): plans[r] = (c_r, beam count, [ROI2] offset of the prefill, invalid slices).  The
+    conditions: every template has generate slots, all of one beam count, with the same invalid slices at each of
+    them in every template; no [ROI2] among the fed tokens; the window inside the template and the cache; dense
+    attention on the K|V cache; at most ops.DECODE_MAX_BATCH rows (and a hidden size the decode kernels take at that
+    batch); not a single row with nucleus sampling (filling_sequence's host loop keeps its torch.multinomial draws);
+    the graph-replayed decode path on."""
+    from .. import ops
+    roi2 = tokenizer['[ROI2]']
+    spans, slice_keys = [], set()
+    ok = (getattr(args, 'is_sparse', 0) == 0 and hasattr(model, 'generate_run') and not torch.is_grad_enabled())
+    for tmpl in tmpls:
+        gen = [i for i, x in enumerate(tmpl) if x < 0]
+        if not gen or len({tmpl[i] for i in gen}) != 1:
+            return [], 0, False
+        _, _, slices = _stretches(tmpl, gen[0], tokenizer)
+        slice_keys.update(tuple((sl.start, sl.stop) for sl in inv) for inv in slices)
+        spans.append((gen[0], gen[-1], -tmpl[gen[0]], slices[0]))
+    S = max(l - f + 1 for f, l, _, _ in spans)
+    plans = []
+    for tmpl, (f, l, nb, inv) in zip(tmpls, spans):
+        c = max(2, l + 1 - S)
+        ok = ok and c <= f and c + S <= len(tmpl) and roi2 not in tmpl[c - 1:c + S - 1]
+        offset = max([i for i, x in enumerate(tmpl[:c - 1]) if x == roi2], default=100000)
+        plans.append((c, nb, offset, inv))
+    tr = getattr(model, 'transformer', None)
+    rows = sum(p[1] for p in plans)
+    ok = (ok and len(slice_keys) == 1 and tr is not None and getattr(tr, 'mems_mode', None) == 'kv'
+          and rows <= ops.DECODE_MAX_BATCH and ops.decode_batch_supported(rows, tr.hidden_size)
+          and max(p[0] for p in plans) - 1 + S <= tr.max_memory_length
+          and not (rows == 1 and args.top_p > 0.0)
+          and _os.environ.get('COGVIEW_B200_FAST_DECODE', '1') != '0'
+          and _os.environ.get('COGVIEW_B200_GRAPH_SAMPLING', '1') != '0')
+    return plans, S, ok
+
+
+def filling_completions(model, seqs, args):
+    """filling_sequences for templates whose given and generate slots differ from template to template (images
+    completed under a different mask each, see generate.complete_images): returns one token tensor [nb, len(seq_c)]
+    per template.  Templates that filling_sequences batches (one layout for all: a context then one generate run, or
+    the interleaved stretches of _stretch_plan) go there.  Otherwise every row runs the window of _completion_plan:
+    its tokens before the window are prefilled alone at batch 1 into its rows of the batch cache
+    (kv_cache.assemble_rows, row_pad), then all rows run S = max_r (l_r - f_r + 1) steps as ONE ragged graph-replayed
+    decode (GPT2Model.generate_run with `forced`): at a generate slot a row keeps its draw, at a given slot the given
+    token replaces it, and either is the next step's input.  A template's nb rows share its prefill and are drawn
+    independently of each other (filling_sequence instead keeps the best-scoring beam at each given token after
+    generated ones); no beam scores are kept.  With top_p > 0 the nucleus filter runs in the sampling kernel.
+    Templates _completion_plan refuses are filled one by one with filling_sequence.  The abs-max LayerNorm scales of
+    the decode step are taken over the whole batch, so a row matches a run of its template alone within bf16
+    tolerance, not bit for bit."""
+    tokenizer = get_tokenizer(args)
+    tmpls = [seq.tolist() for seq in seqs]
+    if len(seqs) > 1 and (_batch_plan(model, tmpls, args, tokenizer)[1]
+                          or _stretch_plan(model, tmpls, args, tokenizer)[1]):
+        return filling_sequences(model, seqs, args)
+    plans, S, ok = _completion_plan(model, tmpls, args, tokenizer)
+    if not ok:
+        return [filling_sequence(model, seq, args) for seq in seqs]
+    from ..mpu import kv_cache
+    device = seqs[0].device
+
+    def prefill(r):
+        c, _, offset, _ = plans[r]
+        tokens, attention_mask, position_ids = get_batch(seqs[r][:c - 1], device, args)
+        position_ids = position_ids.clone()
+        position_ids[position_ids > offset] -= offset
+        _, *mems = model(tokens, position_ids, attention_mask, None, None, 0, logits_last_only=True)
+        return mems
+    mems, row_pad = kv_cache.assemble_rows(model.transformer, [p[0] - 1 for p in plans], [p[1] for p in plans], S,
+                                           prefill)
+    rows = [(tmpl, c, offset) for tmpl, (c, nb, offset, _) in zip(tmpls, plans) for _ in range(nb)]
+    last = torch.tensor([[tmpl[c - 1]] for tmpl, c, _ in rows], dtype=torch.long, device=device)
+    first_pos = [c - 1 - offset if c - 1 > offset else c - 1 for _, c, offset in rows]
+    forced = torch.tensor([[max(x, -1) for x in tmpl[c:c + S]] for tmpl, c, _ in rows], dtype=torch.long,
+                          device=device)
+    res = model.generate_run(last, first_pos, mems, S, args.temperature, args.top_k, plans[0][3], row_pad=row_pad,
+                             top_p=args.top_p, forced=forced)
+    if res is None:
+        raise RuntimeError('filling_completions: the decode batch of %d rows was refused' % len(rows))
+    new_tokens = res[0].to(device)
+    out, r0 = [], 0
+    for seq, (c, nb, _, _) in zip(seqs, plans):
+        filled = seq.view(1, -1).repeat(nb, 1)
+        filled[:, c:c + S] = new_tokens[r0:r0 + nb]
+        out.append(filled)
+        r0 += nb
+    return out
+
+
 def _shared_plan(model, tmpls, args, tokenizer):
     """_batch_plan, and whether filling_shared_prompts can run the templates: _batch_plan's conditions (for one
     template too), every context of the same length, and a model with shared_run."""

@@ -174,7 +174,7 @@ GPT2Model._fast_decode = _fast_decode_impl
 
 
 def _generate_run_impl(self, last_tokens, first_pos, mems, n_steps, temperature, top_k, invalid_slices, sparse=None,
-                       row_pad=None, top_p=0.0):
+                       row_pad=None, top_p=0.0, forced=None):
     """n_steps sampled tokens in a row on the K|V cache — the inner loop of generation/sampling.py:147-183 for a
     stretch of the template that is all 'generate' slots — with the sampling tail inside the replayed CUDA graph
     (mpu/decode.py sample_run).  Returns None when the fast path does not apply, else
@@ -185,7 +185,11 @@ def _generate_run_impl(self, last_tokens, first_pos, mems, n_steps, temperature,
     first_pos is one position for every row, or one per row (a sequence or 1-D tensor of b positions).
     row_pad (int32 [b] on the device, from mpu/kv_cache.py assemble): row i of `mems` holds mems[0].size(1) - row_pad[i]
     tokens — rows of prompts of different lengths in one run (not with sparse).
-    top_p > 0 adds nucleus filtering after top-k (generation/sampling.py:34-47) to the sampling tail."""
+    top_p > 0 adds nucleus filtering after top-k (generation/sampling.py:34-47) to the sampling tail.
+    forced (int64 [b, n_steps] or None; not with sparse): where forced[i, j] >= 0, that given token replaces row i's
+    draw at step j, in the returned tokens and as the input of step j + 1 (generation.sampling.filling_completions:
+    given codes inside a completed region).  The log-probabilities of such rows include the replaced draws and mean
+    nothing."""
     tr = self.transformer
     b = last_tokens.shape[0]
     if (not mems or tr.mems_mode != 'kv' or tr.max_memory_length <= 0 or torch.is_grad_enabled()
@@ -207,10 +211,11 @@ def _generate_run_impl(self, last_tokens, first_pos, mems, n_steps, temperature,
     else:
         pos = torch.full((b, 1), int(first_pos), dtype=torch.long, device=last_tokens.device)
     # sparse inference: cv_sparse_plan is written for at most 16 sequences
-    if sparse is not None and (b > ops.DECODE_SMALL_MAX_BATCH or tr.max_memory_length > 4096 or row_pad is not None):
+    if sparse is not None and (b > ops.DECODE_SMALL_MAX_BATCH or tr.max_memory_length > 4096 or row_pad is not None
+                               or forced is not None):
         return None
     new_tokens, logp = runner.sample_run(last_tokens.reshape(b, 1), pos, caches.t, n_steps, temperature, top_k,
-                                         invalid_slices, sparse=sparse, row_pad=row_pad, top_p=top_p)
+                                         invalid_slices, sparse=sparse, row_pad=row_pad, top_p=top_p, forced=forced)
     return new_tokens, logp, caches.views()
 
 

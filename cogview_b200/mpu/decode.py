@@ -65,6 +65,7 @@ class DecodeRunner:
         self.score_acc = torch.zeros(self.b, dtype=torch.float32, device=dev)
         self.seed_dev = torch.zeros(1, dtype=torch.int64, device=dev)
         self.done = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.forced = None               # given tokens of a run with forced slots (sample_run)
         # sparse inference on the device (is_sparse == 2): text flags of every position, the per-layer key index lists of
         # the current step (cv_sparse_plan) and their common length
         self.sparse = None               # dict(n_img) while a sparse run is being captured / replayed
@@ -208,7 +209,8 @@ class DecodeRunner:
         top-k (generation/sampling.py:24-33), top-p (:34-47), softmax, multinomial draw, beam log-probability — and the
         hand-over of the sampled token to the next step, all through device-side state.  With the fused kernel the
         tail is ONE launch (cv_sample_topk, with the nucleus filter when top_p > 0; own counter-based generator);
-        COGVIEW_B200_FUSED_SAMPLING=0 keeps the reference's torch operations (torch.multinomial's generator) instead."""
+        COGVIEW_B200_FUSED_SAMPLING=0 keeps the reference's torch operations (torch.multinomial's generator) instead.
+        In a run with forced slots (key[6]) the row's given token then replaces the draw."""
         temperature, top_k, inv = key[:3]
         top_p = key[5]
         logits = self._run()
@@ -220,24 +222,32 @@ class DecodeRunner:
             ops.sample_topk(logits, temperature, top_k, valid, seed_dev=self.seed_dev, step=self.stepc,
                             next_ids=self.ids, out_tokens=self.out_buf, score_acc=self.score_acc, pos=self.pos,
                             cur_len=self.cur_len, done=self.done, top_p=top_p)
-            return
-        logits = logits.clone()
-        logits.div_(temperature)
-        for a, z in inv:
-            logits[:, a:z] = -float('Inf')
-        if top_k > 0:
-            kth = torch.topk(logits, top_k)[0][..., -1, None]
-            logits.masked_fill_(logits < kth, -float('Inf'))
-        if top_p > 0.0:
-            top_p_logits(logits, top_p)
-        probs = F.softmax(logits, dim=-1)
-        prev = torch.multinomial(probs, num_samples=1)
-        self.score_acc.add_(torch.log(torch.gather(probs, 1, prev)[:, 0]))
-        self.out_buf.scatter_(1, self.stepc.expand(self.b, 1), prev)
-        self.stepc.add_(1)
-        self.ids.copy_(prev)
-        self.pos.add_(1)
-        self.cur_len.add_(1)
+        else:
+            logits = logits.clone()
+            logits.div_(temperature)
+            for a, z in inv:
+                logits[:, a:z] = -float('Inf')
+            if top_k > 0:
+                kth = torch.topk(logits, top_k)[0][..., -1, None]
+                logits.masked_fill_(logits < kth, -float('Inf'))
+            if top_p > 0.0:
+                top_p_logits(logits, top_p)
+            probs = F.softmax(logits, dim=-1)
+            prev = torch.multinomial(probs, num_samples=1)
+            self.score_acc.add_(torch.log(torch.gather(probs, 1, prev)[:, 0]))
+            self.out_buf.scatter_(1, self.stepc.expand(self.b, 1), prev)
+            self.stepc.add_(1)
+            self.ids.copy_(prev)
+            self.pos.add_(1)
+            self.cur_len.add_(1)
+        if key[6]:
+            # a given token replaces the draw of its step, in the output and as the next step's input; position and
+            # cache length have advanced as for a draw (the tail above has already moved stepc past this step)
+            at = (self.stepc - 1).expand(self.b, 1)
+            given = self.forced.gather(1, at)
+            tok = torch.where(given >= 0, given, self.ids)
+            self.ids.copy_(tok)
+            self.out_buf.scatter_(1, at, tok)
 
     def _reset_run(self, ids, pos, t):
         self.ids.copy_(ids)
@@ -253,23 +263,32 @@ class DecodeRunner:
             self.plan_err.zero_()
 
     def sample_run(self, ids, pos, t, n_steps, temperature, top_k, invalid_slices, sparse=None, row_pad=None,
-                   top_p=0.0):
+                   top_p=0.0, forced=None):
         """n_steps tokens starting from `ids` ([b, 1], at positions `pos`, t tokens cached).  One graph replay per
         token.  Returns (tokens [b, n_steps] int64, summed log-probabilities [b] fp32).
         top_p > 0: nucleus filtering after top-k.
         sparse: None, or dict(n_img=..., tokens=[b, t + 1] every token so far) for is_sparse == 2.
         row_pad: None, or int32 [b] on the device: row i holds t - row_pad[i] cached tokens (ragged mode; not with
-        sparse).  In shared mode t is the suffix length and t + n_steps must fit the suffix cache."""
+        sparse).  In shared mode t is the suffix length and t + n_steps must fit the suffix cache.
+        forced: None, or int64 [b, n_steps]: where forced[i, j] >= 0 that token replaces row i's draw at step j, in
+        the returned tokens and as the next step's input (-1: keep the draw).  The draw is still made, so the summed
+        log-probabilities include draws that were replaced and mean nothing for such rows.  Not with sparse or in
+        shared mode."""
         assert sparse is None or row_pad is None
         assert not self.shared or (sparse is None and t + n_steps <= self.caches.maxlen)
+        assert forced is None or (sparse is None and not self.shared and forced.shape == (self.b, n_steps))
         self._check_params()
         self.last_t = t + n_steps
         vocab = self.model.word_embeddings.weight.shape[0]
         key = (float(temperature), int(top_k), tuple(sl.indices(vocab)[:2] for sl in invalid_slices),
-               None if sparse is None else int(sparse['n_img']), row_pad is not None, float(top_p))
+               None if sparse is None else int(sparse['n_img']), row_pad is not None, float(top_p), forced is not None)
         if self.shared:
             key += (self._mode(),)
         assert n_steps <= self.out_buf.shape[1]
+        if forced is not None:
+            if self.forced is None:          # static: the captured graphs read it
+                self.forced = torch.full_like(self.out_buf, -1)
+            self.forced[:, :n_steps].copy_(forced)
         self._set_rows(row_pad)
         self.sparse = None
         if sparse is not None:
