@@ -219,7 +219,8 @@ def test_token_logprobs_keep_no_memory(ops, small_tok):
     sampling.inverse_prompt_scores(m, q, _Args)
     assert tr.__dict__.get("_kv_pool") == pool and tr._kv is kv
     for k, v in pool.items():
-        assert tr._kv_pool[k] is v and torch.equal(v.buf, bufs[k])
+        # bit for bit: the slots no forward has written hold whatever the allocator left, NaN patterns included
+        assert tr._kv_pool[k] is v and torch.equal(v.buf.view(torch.int16), bufs[k].view(torch.int16))
     with pytest.raises(RuntimeError):
         m.token_logprobs(q, torch.arange(q.shape[1], device="cuda").view(1, -1), 0,
                          torch.tensor([1027], device="cuda"), q[0, 1028:1029], vocab_begin=8192)
