@@ -3,11 +3,10 @@ mpu/sparse_transformer.py:675-725, :629-650, pivot mask :491-496 / :569) — cv_
 
 * forward against tests/golden/attention.npz:sparse_train, the UNMODIFIED reference's output (s = 512, w = 64,
   times = 3, 96 pivots, 2 x 3 heads), and against the oracle restatement on bf16-rounded inputs;
-* backward (dq, dk, dv) against the oracle's autograd through O.sparse_attention with the reference's own
-  rmask-gathered pivot mask, at the golden shape and at the CogView-sr shape (s = 4096, w = 128, times = 6, 768 pivots);
 * a 2-layer GPT2Model training step with is_sparse = 1 (fresh pivots per checkpointed layer in the reference's
   random.sample order) against the oracle evaluated with the same pivots.
-Tolerances (bf16 tensor-core math vs the fp32 oracle): 2e-2 of the output scale forward, 4e-2 of each gradient's scale."""
+Tolerances (bf16 tensor-core math vs the fp32 oracle): 2e-2 of the output scale forward, 4e-2 of each gradient's scale.
+The kernels themselves are bounded element by element in tests/test_attention_sparse_gpu.py."""
 import os
 import random
 
@@ -26,14 +25,6 @@ def _rmask(s, w, times):
     tmp = torch.ones((g - times + 1, w, w))
     tmp = torch.tril(1 - torch.block_diag(*tmp))
     return torch.nn.functional.pad(tmp, (0, (times - 1) * w, (times - 1) * w, 0))
-
-
-def _pivots(b, s, n_piv, txt_n, seed):
-    random.seed(seed)
-    return torch.stack([
-        torch.cat((torch.arange(0, txt_n[i]),
-                   torch.tensor(random.sample(range(txt_n[i], s), n_piv - txt_n[i]), dtype=torch.long)))
-        for i in range(b)])
 
 
 def test_sparse_forward_matches_reference_golden(golden_dir):
@@ -55,42 +46,6 @@ def test_sparse_forward_matches_reference_golden(golden_dir):
     pam = _rmask(s, w, times).expand(b, s, s).gather(dim=-1, index=pivot_idx.unsqueeze(1).expand(b, s, n_piv))
     o = O.sparse_attention(qb, kb, vb, pivot_idx, pam, w, times)
     assert (out - o).abs().max().item() < 1e-2 * o.abs().max().item()
-
-
-@pytest.mark.parametrize("b,nh,s,w,times,n_piv,txt", [(2, 3, 512, 64, 3, 96, (48, 20)), (1, 2, 1024, 128, 6, 200, (64,)),
-                                                     (1, 2, 4096, 128, 6, 768, (100,)), (2, 1, 256, 128, 2, 40, (0, 7)),
-                                                     (1, 1, 768, 128, 6, 64, (30,))])
-def test_sparse_forward_backward_match_oracle_autograd(b, nh, s, w, times, n_piv, txt):
-    from cogview_b200 import ops
-    gen = torch.Generator().manual_seed(s + n_piv)
-    h = nh * 64
-    qkv = torch.randn((b, s, 3 * h), generator=gen).bfloat16()
-    d_out = (torch.randn((b, s, h), generator=gen) * 0.5).bfloat16()
-    pivot_idx = _pivots(b, s, n_piv, txt, seed=99)
-    qc = qkv.cuda()
-    ctx, lse = ops.attn_sparse_fwd(qc[..., :h], qc[..., h:2 * h], qc[..., 2 * h:], nh, pivot_idx.cuda(), w, times,
-                                   want_lse=True)
-    dqkv = ops.attn_sparse_bwd(qc[..., :h], qc[..., h:2 * h], qc[..., 2 * h:], ctx, d_out.cuda(), lse, nh,
-                               pivot_idx.cuda(), w, times).float().cpu()
-    torch.cuda.synchronize()
-
-    def heads_first(t):
-        return t.float().view(b, s, nh, 64).permute(0, 2, 1, 3).contiguous()
-    q, k, v = (heads_first(qkv[..., i * h:(i + 1) * h]).requires_grad_(True) for i in range(3))
-    pam = _rmask(s, w, times).expand(b, s, s).gather(dim=-1, index=pivot_idx.unsqueeze(1).expand(b, s, n_piv))
-    torch.set_num_threads(max(1, min(16, os.cpu_count() or 1)))
-    o = O.sparse_attention(q, k, v, pivot_idx, pam, w, times)
-    o.backward(heads_first(d_out))
-    o_tok = o.detach().permute(0, 2, 1, 3).reshape(b, s, h)
-    err = (ctx.float().cpu() - o_tok).abs().max().item() / o_tok.abs().max().item()
-    print("s=%d w=%d x%d piv=%d: fwd rel err %.3e" % (s, w, times, n_piv, err))
-    assert err < 2e-2
-    for name, got, ref in (("dq", dqkv[..., :h], q.grad), ("dk", dqkv[..., h:2 * h], k.grad),
-                           ("dv", dqkv[..., 2 * h:], v.grad)):
-        ref_tok = ref.permute(0, 2, 1, 3).reshape(b, s, h)
-        e = (got - ref_tok).abs().max().item() / ref_tok.abs().max().item()
-        print("   %s rel err %.3e" % (name, e))
-        assert e < 4e-2, (name, e)
 
 
 def test_model_sparse_training_step_matches_oracle():

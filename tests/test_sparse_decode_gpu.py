@@ -77,37 +77,6 @@ def test_sparse_plan_structure_and_freshness():
     assert (freq - p).abs().max().item() < 6 * math.sqrt(p * (1 - p) / draws)      # no position favoured
 
 
-@pytest.mark.parametrize("b,heads,t,n,nsplit", [(2, 4, 300, 150, 1), (4, 40, 1000, 896, 8), (1, 8, 64, 65, 4)])
-def test_attn_decode_gather_matches_softmax_over_the_gathered_keys(b, heads, t, n, nsplit):
-    from cogview_b200 import ops
-    h = heads * 64
-    g = torch.Generator().manual_seed(t)
-    cache = (torch.randn((b, t + 8, 2 * h), generator=g) * 0.5).to(torch.bfloat16)
-    qkv = (torch.randn((b, 3 * h), generator=g) * 0.5).to(torch.bfloat16)
-    idx = torch.stack([torch.cat((torch.randperm(t, generator=g)[:n - 1].sort().values, torch.tensor([t]))) for _ in range(b)])
-    cache_dev = cache.cuda()
-    nmax = n + 5
-    idx_dev = torch.zeros((b, nmax), dtype=torch.int32, device="cuda")
-    idx_dev[:, :n] = idx.to(torch.int32).cuda()
-    out = ops.attn_decode_gather(qkv.cuda(), cache_dev, heads, torch.tensor([t], dtype=torch.int32, device="cuda"), idx_dev,
-                                 torch.tensor([n], dtype=torch.int32, device="cuda"), nsplit=nsplit)
-    torch.cuda.synchronize()
-    # the new token's K | V were appended at position t
-    assert torch.equal(cache_dev[:, t, :h].cpu(), qkv[:, h:2 * h]) and torch.equal(cache_dev[:, t, h:].cpu(), qkv[:, 2 * h:])
-    full = cache.clone().float()
-    full[:, t, :h] = qkv[:, h:2 * h].float()
-    full[:, t, h:] = qkv[:, 2 * h:].float()
-    q = qkv[:, :h].float().view(b, heads, 1, 64)
-    ref = torch.empty((b, h))
-    for i in range(b):
-        kk = full[i, idx[i], :h].view(n, heads, 64).permute(1, 0, 2)
-        vv = full[i, idx[i], h:].view(n, heads, 64).permute(1, 0, 2)
-        pr = torch.softmax(q[i] @ kk.transpose(1, 2) / 8.0, -1)
-        ref[i] = (pr @ vv).permute(1, 0, 2).reshape(h)
-    err = (out.float().cpu() - ref).abs().max().item()
-    assert err < 2e-2 * ref.abs().max().item(), err
-
-
 def _fill(is_sparse, num_pivot, monkeypatch, pivots="device", text_gen=False):
     """Greedy filling of 60 tokens after a short context with a 4 x 4 = 16-key window: image tokens after [BOI1], or text
     tokens (no [BOI1] in the context: generation/sampling.py starts in the text vocabulary) when text_gen."""

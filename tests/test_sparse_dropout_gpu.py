@@ -1,11 +1,11 @@
 """Attention-probability dropout of sparse TRAINING attention (is_sparse = 1; the reference applies attention_dropout to
 the joint pivot + window probabilities, mpu/sparse_transformer.py:150, :719-721) — cv_attn_sparse_fwd /
 cv_attn_sparse_bwd with dropout_p > 0.  As for the dense sites (tests/test_dropout_gpu.py) bitwise parity with torch's
-generator is not defined; these tests pin the semantics: the kernels against the oracle run with the kernels' own keep
-bits, the keep statistics, and mask replay under activation checkpointing.
-Tolerances as tests/test_sparse_attention_gpu.py: 2e-2 of the output scale forward, 4e-2 of each gradient's scale."""
+generator is not defined; these tests pin the semantics: the keep statistics, mask replay under activation
+checkpointing, and a model step against the oracle run with the kernels' own keep bits (2e-2 of the logit scale, 6e-2 of
+each weight gradient's scale).  The kernels with dropout are bounded element by element against the same keep bits in
+tests/test_attention_sparse_gpu.py."""
 import functools
-import os
 import random
 
 import pytest
@@ -32,59 +32,6 @@ def _rmask(s, w, times):
     tmp = torch.ones((g - times + 1, w, w))
     tmp = torch.tril(1 - torch.block_diag(*tmp))
     return torch.nn.functional.pad(tmp, (0, (times - 1) * w, (times - 1) * w, 0))
-
-
-def _pam(pivot_idx, s, w, times):
-    b, n_piv = pivot_idx.shape
-    return _rmask(s, w, times).expand(b, s, s).gather(dim=-1, index=pivot_idx.unsqueeze(1).expand(b, s, n_piv))
-
-
-@pytest.mark.parametrize("b,nh,s,w,times,n_piv,txt", [(2, 3, 512, 64, 3, 96, (48, 20)), (1, 2, 1024, 128, 6, 200, (64,)),
-                                                     (1, 2, 4096, 128, 6, 768, (100,)), (2, 1, 256, 128, 2, 40, (0, 7))])
-def test_sparse_dropout_forward_backward_match_oracle(b, nh, s, w, times, n_piv, txt):
-    from cogview_b200 import ops
-    gen = torch.Generator().manual_seed(s + n_piv + 1)
-    h = nh * 64
-    qkv = torch.randn((b, s, 3 * h), generator=gen).bfloat16()
-    d_out = (torch.randn((b, s, h), generator=gen) * 0.5).bfloat16()
-    pivot_idx = _pivots(b, s, n_piv, txt, seed=99)
-    qc, pc = qkv.cuda(), pivot_idx.cuda()
-    args = (qc[..., :h], qc[..., h:2 * h], qc[..., 2 * h:], nh, pc, w, times)
-    ctx, lse, mask = ops.attn_sparse_fwd(*args, want_lse=True, dropout=(P, 1234, 7))
-    dqkv = ops.attn_sparse_bwd(*args[:3], ctx, d_out.cuda(), lse, nh, pc, w, times, dropout_p=P,
-                               drop_mask=mask).float().cpu()
-    # dropout off: the existing kernel, bit for bit
-    assert torch.equal(ops.attn_sparse_fwd(*args, dropout=None), ops.attn_sparse_fwd(*args))
-    _, mask2 = ops.attn_sparse_fwd(*args, dropout=(P, 1234, 8))
-    torch.cuda.synchronize()
-
-    fwd, bwd = R.decode_keep(mask, b, nh, s, n_piv, w, times)
-    vis = R.visible(s, n_piv, w, times, pivot_idx).unsqueeze(1).expand_as(fwd)
-    assert (fwd[vis] >= 0).all() and (bwd[vis] >= 0).all(), "a visible pair has no keep bit"
-    both = (fwd >= 0) & (bwd >= 0)
-    assert torch.equal(fwd[both], bwd[both]), "forward and backward layouts disagree"
-    fwd2, _ = R.decode_keep(mask2, b, nh, s, n_piv, w, times)
-    assert (fwd2[vis] != fwd[vis]).float().mean().item() > 0.1          # another site, another mask
-    rate = fwd[vis].float().mean().item()
-    print("s=%d w=%d x%d piv=%d: keep rate over visible pairs %.4f" % (s, w, times, n_piv, rate))
-
-    def heads_first(t):
-        return t.float().view(b, s, nh, 64).permute(0, 2, 1, 3).contiguous()
-    q, k, v = (heads_first(qkv[..., i * h:(i + 1) * h]).requires_grad_(True) for i in range(3))
-    keep = R.to_reference_layout(fwd, s, n_piv, w, times)
-    torch.set_num_threads(max(1, min(16, os.cpu_count() or 1)))
-    o = R.sparse_attention_keep(q, k, v, pivot_idx, _pam(pivot_idx, s, w, times), w, times, keep=keep, dropout_p=P)
-    o.backward(heads_first(d_out))
-    o_tok = o.detach().permute(0, 2, 1, 3).reshape(b, s, h)
-    err = (ctx.float().cpu() - o_tok).abs().max().item() / o_tok.abs().max().item()
-    print("   fwd rel err %.3e" % err)
-    assert err < 2e-2
-    for name, got, ref in (("dq", dqkv[..., :h], q.grad), ("dk", dqkv[..., h:2 * h], k.grad),
-                           ("dv", dqkv[..., 2 * h:], v.grad)):
-        ref_tok = ref.permute(0, 2, 1, 3).reshape(b, s, h)
-        e = (got - ref_tok).abs().max().item() / ref_tok.abs().max().item()
-        print("   %s rel err %.3e" % (name, e))
-        assert e < 4e-2, (name, e)
 
 
 def test_sparse_dropout_mask_statistics():
